@@ -9,7 +9,7 @@ Module classes and parameter names mirror the reference so that its checkpoints 
   TransformerNet                               InvPT/models/transformer_net.py:12-38
 
 The modules own parameters and expose the reference's forward signatures; all arithmetic runs in libmtt_sm90.so
-through `ops` (conventions: taskprompter.py):
+through `ops` (the plan lifecycle and per-module weight caches: plans.py):
 
   TransformerNet.forward(x)              -> {task: [B,n,H,W], 'inter_preds': {...}}   the fused path, ONE CUDA graph
   VisionTransformer.forward(x)           -> (x [B,P,C], [4 x [B,P,C]])                 vit.py:332-361
@@ -27,8 +27,9 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .taskprompter import (PARITY, Mlp, PatchEmbed, _cached, _check_input, _dev_ctx, _f32, _plan_for, _Streams,
-                           _trunc_normal_, _version)
+from .plans import (Plan, _cached, _check_input, _dev_ctx, _f32, _lin, _pack_stem, _pack_vit_block, _plan_for,
+                    _predict_outputs)
+from .taskprompter import PARITY, Mlp, PatchEmbed, _trunc_normal_
 
 
 # --------------------------------------------------------------------------------------------
@@ -115,9 +116,7 @@ class MLPHead(nn.Module):
         B, Cin, h, w = x.shape
         dev, ns = x.device, self.nsplit
         with _dev_ctx(dev):
-            lp = _cached(self, ("pack", dev, ns), lambda: (
-                ops.pack_weight(_f32(self.linear_pred.weight, dev).reshape(self.linear_pred.weight.shape[0], -1), ns),
-                _f32(self.linear_pred.bias, dev)))
+            lp = _pack_mlp_head(self, dev, ns)
             n = self.linear_pred.weight.shape[0]
             a = ops.Split(B * h * w, Cin, dev, ns)
             ops.nchw_to_nhwc_split(x.contiguous(), a)
@@ -126,6 +125,11 @@ class MLPHead(nn.Module):
             out = torch.empty(B, n, h, w, device=dev, dtype=torch.float32)
             ops.nhwc_to_nchw(y, y.stride(0), B, n, h, w, out)
             return out
+
+
+def _pack_mlp_head(hd, device, ns):
+    """MLPHead.linear_pred as (packed weight, bias), cached on the head (shared by MLPHead.forward and the plans)."""
+    return _cached(hd, ("pack", device, ns), lambda: _lin(hd.linear_pred, device, ns))
 
 
 class UpEmbed(nn.Module):
@@ -296,30 +300,6 @@ class TransformerNet(nn.Module):
 # --------------------------------------------------------------------------------------------
 # the fused forward
 # --------------------------------------------------------------------------------------------
-def _pack_vit(bb, device, ns):
-    """Patch embedding, cls / position rows, the ViT blocks and the final norm (vit.py:172-351)."""
-    def build():
-        f = lambda t: _f32(t, device)
-        W = SimpleNamespace()
-        W.pe_w = ops.pack_weight(f(bb.patch_embed.proj.weight).reshape(bb.embed_dim, -1), ns)
-        W.pe_b = f(bb.patch_embed.proj.bias)
-        W.pos = f(bb.pos_embed)[0, 1:].contiguous()
-        W.cls = (f(bb.cls_token)[0] + f(bb.pos_embed)[0, :1]).contiguous()      # vit.py:334-339, row 0
-        W.blocks = []
-        for blk in bb.blocks:
-            w = SimpleNamespace()
-            w.n1w, w.n1b, w.n2w, w.n2b = f(blk.norm1.weight), f(blk.norm1.bias), f(blk.norm2.weight), f(blk.norm2.bias)
-            w.eps = blk.norm1.eps
-            w.qkv, w.qkv_b = ops.pack_weight(f(blk.attn.qkv.weight), ns), f(blk.attn.qkv.bias)
-            w.proj, w.proj_b = ops.pack_weight(f(blk.attn.proj.weight), ns), f(blk.attn.proj.bias)
-            w.fc1, w.fc1_b = ops.pack_weight(f(blk.mlp.fc1.weight), ns), f(blk.mlp.fc1.bias)
-            w.fc2, w.fc2_b = ops.pack_weight(f(blk.mlp.fc2.weight), ns), f(blk.mlp.fc2.bias)
-            W.blocks.append(w)
-        W.nw, W.nb, W.neps = f(bb.norm.weight), f(bb.norm.bias), bb.norm.eps
-        return W
-    return _cached(bb, ("pack", device, ns), build)
-
-
 def _pack_decoder(dec, tasks, device, ns):
     """scale_embed, preliminary decoders and intermediate heads (transformer_decoder.py:18-98), BatchNorm folded."""
     def build():
@@ -336,8 +316,7 @@ def _pack_decoder(dec, tasks, device, ns):
             pd = dec.preliminary_decoder[t]
             tw.pd0, tw.pd0_b = ops.pack_conv_weight(f(pd[0].conv.weight), None, pd[0].bn1, ns)
             tw.pd1, tw.pd1_b = ops.pack_conv_weight(f(pd[1].conv.weight), None, pd[1].bn1, ns)
-            ih = dec.intermediate_head[t]
-            tw.ih, tw.ih_b = ops.pack_weight(f(ih.weight).reshape(ih.weight.shape[0], -1), ns), f(ih.bias)
+            tw.ih, tw.ih_b = _lin(dec.intermediate_head[t], device, ns)
             W.tasks.append(tw)
         return W
     return _cached(dec, ("pack_dec", device, ns, tuple(tasks)), build)
@@ -351,8 +330,7 @@ def _pack_invpt(inv, tasks, device, ns):
         W = SimpleNamespace(tasks=[], stages=[])
         for t in tasks:
             tw = SimpleNamespace()
-            mx = inv.mix_proj[t][0]
-            tw.mix, tw.mix_b = ops.pack_weight(f(mx.weight).reshape(mx.weight.shape[0], -1), ns), f(mx.bias)
+            tw.mix, tw.mix_b = _lin(inv.mix_proj[t][0], device, ns)
             tw.mt, tw.mt_b = ops.pack_conv_weight(f(inv.mt_proj[t][0].weight), inv.mt_proj[t][0].bias, inv.mt_proj[t][1], ns)
             W.tasks.append(tw)
         for i, st in enumerate(inv.invpt_stages):
@@ -374,46 +352,42 @@ def _pack_invpt(inv, tasks, device, ns):
                 qw.append((f(cq.conv.weight) * sc.reshape(-1, 1, 1, 1)).reshape(dims[i], 9))
                 qb.append(f(cq.bn.bias) - f(cq.bn.running_mean) * sc)
             sw.dw_w, sw.dw_b = torch.stack(qw).contiguous(), torch.stack(qb).contiguous()
-            for nm in ("proj_q", "proj_k", "proj_v", "proj"):
-                lin = getattr(blk.attn, nm)
-                setattr(sw, nm, ops.pack_weight(f(lin.weight), ns))
-                setattr(sw, nm + "_b", f(lin.bias))
+            sw.proj_q, sw.proj_q_b = _lin(blk.attn.proj_q, device, ns)
+            sw.proj_k, sw.proj_k_b = _lin(blk.attn.proj_k, device, ns)
+            sw.proj_v, sw.proj_v_b = _lin(blk.attn.proj_v, device, ns)
+            sw.proj, sw.proj_b = _lin(blk.attn.proj, device, ns)
             sw.fuse_w = f(blk.attn.fuse_attn.weight).reshape(2, 4).contiguous()
             sw.fuse_b = f(blk.attn.fuse_attn.bias)
-            sw.fc1, sw.fc1_b = ops.pack_weight(f(blk.mlp.fc1.weight), ns), f(blk.mlp.fc1.bias)
-            sw.fc2, sw.fc2_b = ops.pack_weight(f(blk.mlp.fc2.weight), ns), f(blk.mlp.fc2.bias)
+            sw.fc1, sw.fc1_b = _lin(blk.mlp.fc1, device, ns)
+            sw.fc2, sw.fc2_b = _lin(blk.mlp.fc2, device, ns)
             sw.nmw, sw.nmb, sw.nmeps = f(inv.norm_mts[i].weight), f(inv.norm_mts[i].bias), inv.norm_mts[i].eps
             if i > 0:
-                sw.redu = [(ops.pack_weight(f(inv.redu_chan[i][k].weight).reshape(dims[0], -1), ns),
-                            f(inv.redu_chan[i][k].bias)) for k in range(T)]
+                sw.redu = [_lin(inv.redu_chan[i][k], device, ns) for k in range(T)]
             W.stages.append(sw)
         return W
     return _cached(inv, ("pack_inv", device, ns, tuple(tasks)), build)
 
 
-class _Plan:
-    """Workspace + launch sequence (+ CUDA graph) for one batch size. mode: "full" / "postproc" = TransformerNet
+class _Plan(Plan):
+    """Geometry, workspace and launch sequence of one InvPT forward. mode: "full" / "postproc" = TransformerNet
     forward / predict; "backbone" = VisionTransformer.forward; "decoder" = TransformerDecoder.forward on given
-    backbone features; "invpt" = InvPT.forward on given task features, preliminary predictions and skips."""
+    backbone features; "invpt" = InvPT.forward on given task features, preliminary predictions and skips (these two
+    take no image: `run(None, graph=False)` after `load_features` / `load_invpt_inputs`)."""
 
     def __init__(self, bb, dec, heads, p, tasks, B, device, nsplit, mode="full", inv=None, hw0=None):
-        ops._L.check(ops._L.load().mtt_device_check(), "mtt_device_check")
-        device = torch.device(device)
+        self.inv = inv if inv is not None else (dec.invpt if dec is not None else None)
+        super().__init__((bb, dec if dec is not None else self.inv, heads), B, device, nsplit, len(tasks))
+        device = self.dev
         self.mode = mode
         self.postproc = mode == "postproc"
         self.bb, self.dec, self.heads, self.p = bb, dec, heads, p
-        self.inv = inv if inv is not None else (dec.invpt if dec is not None else None)
-        self.B, self.dev, self.ns = B, device, nsplit
         self.tasks = list(tasks)
         self.T = T = len(self.tasks)
-        self.graph = None
-        self.static_in = None
-        self.streams = _Streams(device, max(T, 1))
         ns = nsplit
         S = lambda r, c, **kw: ops.Split(r, c, device, ns, **kw)
         z = lambda *s: torch.zeros(*s, device=device, dtype=torch.float32)
         with _dev_ctx(device):
-            self._pack()
+            self._repack()
             if bb is not None:
                 self.C = C = bb.embed_dim
                 self.H = bb.num_heads
@@ -522,7 +496,6 @@ class _Plan:
                 if mode == "decoder":
                     self.inter_nchw = {t: z(B, n, h0, w0) for t, n in zip(self.tasks, self.n_out)}
                     self.out["inter_pred"] = self.inter_nchw
-                self.out_inter = None
                 return
             self.pred = [z(tt, ops.round_up(n, 4)) for n in self.n_out]
             oh, ow = self.img
@@ -530,36 +503,21 @@ class _Plan:
                 self.out = {t: z(B, n, oh, ow) for t, n in zip(self.tasks, self.n_out)}
                 self.out_inter = {t: z(B, n, oh, ow) for t, n in zip(self.tasks, self.n_out)}
             else:
-                self.out, self.out_inter = {}, None
-                for t in self.tasks:
-                    kind = ops.POSTPROC_KIND[t]
-                    shape = {0: (B, oh, ow), 1: (B, oh, ow), 2: (B, oh, ow), 3: (B, oh, ow, 3), 4: (B, oh, ow, 1)}[kind]
-                    self.out[t] = torch.zeros(shape, device=device, dtype=torch.int64 if kind == 0 else torch.float32)
+                self.out = _predict_outputs(self.tasks, B, (oh, ow), device)
 
     def _pack(self):
-        dev, ns = self.dev, self.ns
-        self.Wv = _pack_vit(self.bb, dev, ns) if self.bb is not None else None
+        bb, dev, ns = self.bb, self.dev, self.ns
+        self.Ws = _pack_stem(bb, dev, ns) if bb is not None else None
+        self.Wb = [_pack_vit_block(blk, dev, ns) for blk in bb.blocks] if bb is not None else None
         self.Wd = _pack_decoder(self.dec, self.tasks, dev, ns) if self.dec is not None else None
         self.Wi = _pack_invpt(self.inv, self.tasks, dev, ns) if self.inv is not None else None
-        self.Wh = None
-        if self.heads is not None:
-            self.Wh = [_cached(self.heads[t], ("pack", dev, ns), lambda t=t: (
-                ops.pack_weight(_f32(self.heads[t].linear_pred.weight, dev).reshape(
-                    self.heads[t].linear_pred.weight.shape[0], -1), ns), _f32(self.heads[t].linear_pred.bias, dev)))
-                for t in self.tasks]
-        self.version = self._ver()
+        self.Wh = [_pack_mlp_head(self.heads[t], dev, ns) for t in self.tasks] if self.heads is not None else None
 
-    def _ver(self):
-        return sum(_version(m) for m in (self.bb, self.dec if self.dec is not None else self.inv, self.heads)
-                   if m is not None)
-
-    @property
-    def serial(self):
-        return self.streams.serial
-
-    @serial.setter
-    def serial(self, v):
-        self.streams.serial = bool(v)
+    def _result(self):
+        out = dict(self.out)
+        if self.mode == "full":
+            out["inter_preds"] = dict(self.out_inter)
+        return out
 
     def _par(self, fn):
         """Run fn(k) for every task k, each on its own side stream forked from / joined to the current
@@ -700,12 +658,12 @@ class _Plan:
                          out_nchw=self.out[self.tasks[k]])                                             # transformer_net.py:35
 
     def _launch_backbone(self, img):
-        B, N, P, C, W = self.B, self.N, self.P, self.C, self.Wv
+        B, N, P, C, W = self.B, self.N, self.P, self.C, self.Ws
         ops.im2col_patch(img, self.patch, self.cols)
         ops.gemm(self.cols, W.pe_w, bias=W.pe_b, residual=W.pos, res_row_mod=P, out_f32=self.xs,
                  regroup=(P, N, 1))                                                                    # vit.py:333,339
         ops.broadcast_rows(W.cls, self.xs, B, N)                                                       # :334-339
-        for idx, w in enumerate(W.blocks):
+        for idx, w in enumerate(self.Wb):
             self._vit_block(w)
             if idx + 1 in self.select:
                 which = self.select.index(idx + 1)
@@ -756,42 +714,6 @@ class _Plan:
             self._launch_decoder_front()
         if self.mode != "backbone":
             self._launch_invpt()
-
-    def run(self, x, graph=True):
-        with _dev_ctx(self.dev):
-            if self._ver() != self.version:      # parameters changed in place: re-pack, re-capture
-                self._pack()
-                self.graph = None
-            if self.mode in ("decoder", "invpt"):
-                self._launch(None)
-                return self.out
-            if tuple(x.shape[1:]) != (3, *self.img) or x.dtype != torch.float32:
-                raise ValueError(f"expected fp32 input [B,3,{self.img[0]},{self.img[1]}], got {tuple(x.shape)} {x.dtype}")
-            if not graph:
-                self._launch(x.contiguous())
-            else:
-                if self.static_in is None:
-                    self.static_in = torch.empty_like(x, memory_format=torch.contiguous_format)
-                self.static_in.copy_(x, non_blocking=True)
-                if self.graph is None:
-                    self._launch(self.static_in)
-                    torch.cuda.synchronize()
-                    g = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(g):
-                        self._launch(self.static_in)
-                    self.graph = g
-                self.graph.replay()
-            out = dict(self.out)
-            if self.mode == "full":
-                out["inter_preds"] = dict(self.out_inter)
-            return out
-
-    def launches_per_forward(self):
-        with _dev_ctx(self.dev):
-            n0 = ops.launch_count()
-            self._launch(self.static_in if self.static_in is not None else
-                         torch.zeros(self.B, 3, *self.img, device=self.dev))
-            return ops.launch_count() - n0
 
 
 def build_from_config(cfg, nsplit=PARITY, use_graph=True):

@@ -10,16 +10,16 @@ checkpoints (`backbone.blocks.{i}.attn.qkv.weight`, `backbone.fea_fuse.{il}.{tas
 The modules OWN parameters and expose the reference's forward signatures; all arithmetic runs in
 libmtt_sm90.so through `ops`:
 
-  TaskPrompterWrapper.forward(x)      -> {task: [B,n_out,H,W]}      the fused path: one `_Plan` (packed weights +
-                                                                    fixed workspace) replayed as ONE CUDA graph
+  TaskPrompterWrapper.forward(x)      -> {task: [B,n_out,H,W]}      the fused path: one `_Plan` (plans.Plan: packed
+                                                                    weights + fixed workspace) replayed as ONE CUDA graph
   TaskPrompter.forward(x)             -> (task_fea {task: [B,f,4h,4w]}, {})      taskprompter.py:392-422
   Block.forward(x, task_prompts)      -> (x, (prompt_logits, raw_chan), task_prompts)   :270-279
   ConvHead / DEConvHead.forward(x)    -> [B,n_out,h,w] / [B,n_out,2h,2w]          :697, :712-715
 
 The sub-module forwards run the SAME kernels eagerly on small private workspaces (NCHW tensors in and out like the
 reference); they exist so that code written against the reference's module boundaries keeps working, the wrapper
-forward is the one to time. Packed weights (split-bf16, BatchNorm folded, tap-major convs) are cached per module,
-device, precision mode and parameter version and shared by every plan / sub-module forward.
+forward is the one to time. The plan lifecycle and the per-module weight caches that every plan and sub-module forward
+shares are in plans.py.
 
 Changes to the reference's internal contract: `Block` returns `(prompt_logits [B,H,T,N], raw_chan [B,T,C,nh,nw])`
 in place of the full [B,H,N,N] attention maps (only those parts are ever consumed, SURVEY.md H4; the logits are
@@ -34,82 +34,10 @@ import torch
 import torch.nn as nn
 
 from . import ops
+from .plans import (Plan, _cached, _check_input, _dev_ctx, _f32, _lin, _pack_stem, _pack_vit_block, _plan_for,
+                    _predict_outputs, _Streams)
 
 PARITY, SPEED = 2, 1  # nsplit: 3-MMA split-bf16 (fp32-grade) vs plain bf16
-MAX_PLANS = 4         # cached plans (workspace + CUDA graph) per module, least recently used is dropped
-
-
-# --------------------------------------------------------------------------------------------
-# per-module caches: packed weights and eager workspaces
-# --------------------------------------------------------------------------------------------
-def _version(mod):
-    return sum(int(q._version) for q in mod.parameters()) + sum(int(b._version) for b in mod.buffers())
-
-
-def _cached(mod, key, build, versioned=True):
-    """build() once per (module, key, parameter version); lives in the module's __dict__ (not a parameter / buffer)."""
-    store = mod.__dict__.setdefault("_mtt_cache", {})
-    ver = _version(mod) if versioned else 0
-    hit = store.get(key)
-    if hit is None or hit[0] != ver:
-        with _dev_ctx(key[1]):
-            hit = (ver, build())
-        store[key] = hit
-    return hit[1]
-
-
-def _dev_ctx(device):
-    """torch.cuda.device(device) for CUDA devices (the C side works on the CURRENT device: streams, kernel attributes,
-    SM count), a no-op otherwise (CPU emulation in the tests)."""
-    import contextlib
-    device = torch.device(device)
-    return torch.cuda.device(device) if device.type == "cuda" else contextlib.nullcontext()
-
-
-def _f32(t, device):
-    return t.detach().to(device=device, dtype=torch.float32).contiguous()
-
-
-def _check_input(mod, x):
-    if mod.training:
-        raise NotImplementedError("mtt_b200: the fused forward is eval-only; call .eval() (backward kernels: "
-                                  "SURVEY.md section 8f N1)")
-    if not x.is_cuda:
-        raise RuntimeError("mtt_b200 has no CPU path: input must be a CUDA tensor on an sm_90a (H100) device")
-    ops._L.check(ops._L.load().mtt_device_check(), "mtt_device_check")
-
-
-class _Streams:
-    """Fork / join of side streams off the current stream (captured into the same CUDA graph)."""
-
-    def __init__(self, dev, n):
-        self.dev, self.n, self.side, self.serial = dev, max(n, 1), None, False
-
-    def fork(self, n):
-        if self.dev.type != "cuda" or self.serial:   # serial: one stream (per-kernel timing)
-            return None, [None] * n
-        if self.side is None:
-            self.side = [torch.cuda.Stream(device=self.dev) for _ in range(self.n)]
-        main = torch.cuda.current_stream()
-        for st in self.side[:n]:
-            st.wait_stream(main)
-        return main, self.side[:n]
-
-    def join(self, main, n):
-        if main is not None:
-            for st in self.side[:n]:
-                main.wait_stream(st)
-
-    def par(self, fns):
-        """Run the callables concurrently, one per side stream."""
-        main, side = self.fork(len(fns))
-        for st, fn in zip(side, fns):
-            if st is None:
-                fn()
-            else:
-                with torch.cuda.stream(st):
-                    fn()
-        self.join(main, len(fns))
 
 
 # --------------------------------------------------------------------------------------------
@@ -139,25 +67,6 @@ class Attention(nn.Module):
         self.proj = nn.Linear(dim, dim)
         self.token_trans = nn.Linear(dim, self.pixel_no)
         self.token_trans1 = nn.Linear(self.pixel_no, dim)
-
-
-def _pack_block(blk, device, ns):
-    """Packed operands of one Block (taskprompter.py:257-268), cached on the module."""
-    def build():
-        f = lambda t: _f32(t, device)
-        w = SimpleNamespace()
-        w.n1w, w.n1b, w.n2w, w.n2b = f(blk.norm1.weight), f(blk.norm1.bias), f(blk.norm2.weight), f(blk.norm2.bias)
-        w.eps = blk.norm1.eps
-        zeros = lambda n: torch.zeros(n, device=device)
-        a = blk.attn
-        w.qkv, w.qkv_b = ops.pack_weight(f(a.qkv.weight), ns), (f(a.qkv.bias) if a.qkv.bias is not None else zeros(3 * a.dim))
-        w.proj, w.proj_b = ops.pack_weight(f(a.proj.weight), ns), f(a.proj.bias)
-        w.tt, w.tt_b = ops.pack_weight(f(a.token_trans.weight), ns), f(a.token_trans.bias)
-        w.tt1, w.tt1_b = ops.pack_weight(f(a.token_trans1.weight), ns), f(a.token_trans1.bias)
-        w.fc1, w.fc1_b = ops.pack_weight(f(blk.mlp.fc1.weight), ns), f(blk.mlp.fc1.bias)
-        w.fc2, w.fc2_b = ops.pack_weight(f(blk.mlp.fc2.weight), ns), f(blk.mlp.fc2.bias)
-        return w
-    return _cached(blk, ("pack", device, ns), build)
 
 
 class _BlockSpace:
@@ -243,7 +152,7 @@ class Block(nn.Module):
             raise ValueError(f"Block: expected x [B,{a.pixel_no},{a.dim}] with head dim 64, got {tuple(x.shape)}")
         dev, ns = x.device, self.nsplit
         with _dev_ctx(dev):
-            w = _pack_block(self, dev, ns)
+            w = _pack_vit_block(self, dev, ns)
             sp = _cached(self, ("space", dev, ns, B, T), lambda: _BlockSpace(
                 B, T, a.resolution[0], a.resolution[1], C, a.num_heads, self.mlp.fc1.out_features, a.chan_nheads, dev,
                 ns), versioned=False)
@@ -360,18 +269,6 @@ class TaskPrompter(nn.Module):
         return {t: v.clone() for t, v in out.items()}, {}
 
 
-def _plan_for(mod, key, build):
-    """LRU cache of plans on `mod` (a plan = workspace + CUDA graph for one batch size; weights are shared)."""
-    plans = mod.__dict__.setdefault("_mtt_plans", {})
-    pl = plans.pop(key, None)
-    if pl is None:
-        pl = build()
-    plans[key] = pl                      # most recently used last
-    while len(plans) > MAX_PLANS:
-        plans.pop(next(iter(plans)))
-    return pl
-
-
 def _pack_head(hd, device, ns):
     """ConvHead (taskprompter.py:688-698) / DEConvHead (:700-715) operands, BatchNorm folded."""
     def build():
@@ -395,8 +292,7 @@ def _pack_head(hd, device, ns):
             hw.mid = hd.mt_proj[0].weight.shape[0]
             hw.mt, hw.mt_b = ops.pack_conv_weight(f(hd.mt_proj[0].weight), hd.mt_proj[0].bias, hd.mt_proj[1], ns)
         hw.cin = hd.mt_proj[0].weight.shape[0] if hw.deconv else hd.mt_proj[0].weight.shape[1]
-        hw.lp, hw.lp_b = ops.pack_weight(f(hd.linear_pred.weight).reshape(hd.linear_pred.weight.shape[0], -1), ns), \
-            f(hd.linear_pred.bias)
+        hw.lp, hw.lp_b = _lin(hd.linear_pred, device, ns)
         hw.n_out = hd.linear_pred.weight.shape[0]
         return hw
     return _cached(hd, ("pack", device, ns), build)
@@ -521,45 +417,38 @@ class TaskPrompterWrapper(nn.Module):
 # --------------------------------------------------------------------------------------------
 # the fused forward
 # --------------------------------------------------------------------------------------------
-def _pack_stem(bb, device, ns):
-    def build():
-        f = lambda t: _f32(t, device)
-        W = SimpleNamespace()
-        W.pe_w = ops.pack_weight(f(bb.patch_embed.proj.weight).reshape(bb.embed_dim, -1), ns)
-        W.pe_b = f(bb.patch_embed.proj.bias)
-        W.pos = f(bb.pos_embed)[0, 1:].contiguous()           # [P, C] (cls slot skipped, :394)
-        W.prompts = f(bb.task_prompts)
-        W.nw, W.nb, W.neps = f(bb.norm.weight), f(bb.norm.bias), bb.norm.eps
-        return W
-    return _cached(bb, ("stem", device, ns), build)
+def _pack_fuse(bb, il, t, device, ns):
+    """fea_decode_spa / fea_decode_chan / fea_fuse of task t at level il (:352-366), for both backbones: fea_fuse[0]'s K
+    laid out like the zero-padded `cat` buffer, fea_fuse[1] folded with its eval BatchNorm."""
+    f = lambda x: _f32(x, device)
+    tw = SimpleNamespace()
+    tw.spa, tw.spa_b = _lin(bb.fea_decode_spa[il][t][0], device, ns)
+    tw.chan, tw.chan_b = _lin(bb.fea_decode_chan[il][t][0], device, ns)
+    fu = bb.fea_fuse[il][t]
+    ff, e = fu[0].weight.shape[0], fu[0].weight.shape[1] // 2
+    e_pad = ops.round_up(e, 8)
+    w0 = f(fu[0].weight).reshape(ff, 2 * e)
+    w0p = torch.zeros(ff, 2 * e_pad, device=device)
+    w0p[:, :e] = w0[:, :e]
+    w0p[:, e_pad:e_pad + e] = w0[:, e:]
+    tw.f0, tw.f0_b = ops.pack_weight(w0p, ns), f(fu[0].bias)
+    tw.f1, tw.f1_b = ops.pack_conv_weight(f(fu[1].weight), fu[1].bias, fu[2], ns)
+    if fu[4].kernel_size == (1, 1):
+        tw.f4, tw.f4_b = _lin(fu[4], device, ns)
+    else:                                                                 # 3x3 in TaskPrompterSwin (TP swin :630)
+        tw.f4, tw.f4_b = ops.pack_conv_weight(f(fu[4].weight), fu[4].bias, None, ns)
+    return tw
 
 
 def _pack_levels(bb, tasks, device, ns):
     """fea_decode_spa / fea_decode_chan / fea_fuse / ctr_attn_conv operands of all 4 levels (:352-366)."""
     def build():
         f = lambda t: _f32(t, device)
-        p = bb.p
-        e, ff, H = p.embed_dim, p.final_embed_dim, bb.num_heads
-        e_pad = ops.round_up(e, 8)
+        H = bb.num_heads
         levels = []
         for il in range(4):
-            lv = SimpleNamespace(tasks=[])
-            for t in tasks:
-                tw = SimpleNamespace()
-                tw.spa = ops.pack_weight(f(bb.fea_decode_spa[il][t][0].weight).reshape(e, -1), ns)
-                tw.spa_b = f(bb.fea_decode_spa[il][t][0].bias)
-                tw.chan = ops.pack_weight(f(bb.fea_decode_chan[il][t][0].weight).reshape(e, -1), ns)
-                tw.chan_b = f(bb.fea_decode_chan[il][t][0].bias)
-                fu = bb.fea_fuse[il][t]
-                w0 = f(fu[0].weight).reshape(ff, 2 * e)
-                w0p = torch.zeros(ff, 2 * e_pad, device=device)   # K laid out like the `cat` buffer
-                w0p[:, :e] = w0[:, :e]
-                w0p[:, e_pad:e_pad + e] = w0[:, e:]
-                tw.f0, tw.f0_b = ops.pack_weight(w0p, ns), f(fu[0].bias)
-                tw.f1, tw.f1_b = ops.pack_conv_weight(f(fu[1].weight), fu[1].bias, fu[2], ns)   # conv3x3 + eval BN
-                tw.f4, tw.f4_b = ops.pack_weight(f(fu[4].weight).reshape(ff, -1), ns), f(fu[4].bias)
-                lv.tasks.append(tw)
-            if p.use_ctr:
+            lv = SimpleNamespace(tasks=[_pack_fuse(bb, il, t, device, ns) for t in tasks])
+            if bb.p.use_ctr:
                 cc = [bb.ctr_attn_conv[il][t] for t in tasks]
                 lv.c0 = torch.stack([f(c[0].weight).reshape(H, H) for c in cc]).contiguous()
                 lv.c0b = torch.stack([f(c[0].bias) for c in cc]).contiguous()
@@ -570,19 +459,18 @@ def _pack_levels(bb, tasks, device, ns):
     return _cached(bb, ("levels", device, ns, tuple(tasks)), build)
 
 
-class _Plan:
-    """Workspace + launch sequence (+ CUDA graph) for one (batch size, device, nsplit, mode); the packed weights are
-    the per-module caches above. mode: "full" = wrapper forward (logits at the output size), "postproc" = predict(),
-    "backbone" = TaskPrompter.forward alone (task features, NCHW)."""
+class _Plan(Plan):
+    """Geometry, workspace and launch sequence of one TaskPrompter (ViT) forward. mode: "full" = wrapper forward
+    (logits at the output size), "postproc" = predict(), "backbone" = TaskPrompter.forward alone (task features,
+    NCHW)."""
 
     def __init__(self, bb, heads, tasks, target, B, device, nsplit, mode="full"):
-        ops._L.check(ops._L.load().mtt_device_check(), "mtt_device_check")
-        device = torch.device(device)
+        super().__init__((bb, heads), B, device, nsplit, len(tasks))
+        device = self.dev
         self.mode = mode
         self.postproc = mode == "postproc"
         p = bb.p
         self.bb, self.heads = bb, heads
-        self.B, self.dev, self.ns = B, device, nsplit
         self.tasks = list(tasks)
         self.T = T = len(self.tasks)
         self.C = C = bb.embed_dim
@@ -602,13 +490,10 @@ class _Plan:
         self.f_ld = ops.round_up(self.f, 8)
         self.use_ctr = bool(p.use_ctr)
         self.target = target
-        self.graph = None
-        self.static_in = None
         ns = nsplit
         e_pad, f = self.e_pad, self.f
         with _dev_ctx(device):
-            self.streams = _Streams(device, max(T, 1))
-            self._pack()
+            self._repack()
             # ---- workspace ------------------------------------------------------------------------------
             S = lambda r, c, **kw: ops.Split(r, c, device, ns, **kw)
             z = lambda *s: torch.zeros(*s, device=device, dtype=torch.float32)
@@ -632,34 +517,23 @@ class _Plan:
             gh4, gw4 = 4 * self.gh, 4 * self.gw
             oh, ow = self.target if self.target is not None else self.img
             self.out_hw = (oh, ow)
-            self.out = {}
             if mode == "backbone":
                 self.hs = None
                 self.out = {t: z(B, f, gh4, gw4) for t in self.tasks}
                 return
             self.hs = [_HeadSpace(hw, B, gh4, gw4, device, ns) for hw in self.Wh]
-            for t, hw, hs in zip(self.tasks, self.Wh, self.hs):
-                if t == "3ddet":                                   # wrapper :34-38: this task is not resized
-                    if self.postproc:
-                        raise ValueError("no get_output post-processing defined for task '3ddet'")
-                    self.out[t] = z(B, hw.n_out, hs.ph, hs.pw)
-                elif not self.postproc:
-                    self.out[t] = z(B, hw.n_out, oh, ow)
-                else:
-                    if t not in ops.POSTPROC_KIND:
-                        raise ValueError(f"no get_output post-processing defined for task {t!r}")
-                    kind = ops.POSTPROC_KIND[t]
-                    shape = {0: (B, oh, ow), 1: (B, oh, ow), 2: (B, oh, ow), 3: (B, oh, ow, 3), 4: (B, oh, ow, 1)}[kind]
-                    self.out[t] = torch.zeros(shape, device=device, dtype=torch.int64 if kind == 0 else torch.float32)
+            if self.postproc:
+                self.out = _predict_outputs(self.tasks, B, (oh, ow), device)
+            else:                                                  # wrapper :34-38: '3ddet' is not resized
+                self.out = {t: z(B, hw.n_out, hs.ph, hs.pw) if t == "3ddet" else z(B, hw.n_out, oh, ow)
+                            for t, hw, hs in zip(self.tasks, self.Wh, self.hs)}
 
     def _pack(self):
-        """(Re)resolve the packed weights from the per-module caches (cheap when nothing changed)."""
         bb, dev, ns = self.bb, self.dev, self.ns
         self.Ws = _pack_stem(bb, dev, ns)
-        self.Wb = [_pack_block(blk, dev, ns) for blk in bb.blocks]
+        self.Wb = [_pack_vit_block(blk, dev, ns) for blk in bb.blocks]
         self.Wl = _pack_levels(bb, self.tasks, dev, ns)
         self.Wh = [_pack_head(self.heads[t], dev, ns) for t in self.tasks] if self.heads is not None else None
-        self.version = _version(bb) + (_version(self.heads) if self.heads is not None else 0)
 
     # -- launch sequence ------------------------------------------------------------------------
     def _level(self, il, x_src):
@@ -724,45 +598,6 @@ class _Plan:
             return
         self.streams.par([lambda ti=ti, t=t, hw=hw, hs=hs: self._head_chain(ti, t, hw, hs)
                           for ti, (t, hw, hs) in enumerate(zip(self.tasks, self.Wh, self.hs))])
-
-    @property
-    def serial(self):
-        return self.streams.serial
-
-    @serial.setter
-    def serial(self, v):
-        self.streams.serial = bool(v)
-
-    def run(self, x, graph=True):
-        if tuple(x.shape[1:]) != (3, *self.img) or x.dtype != torch.float32:
-            raise ValueError(f"expected fp32 input [B,3,{self.img[0]},{self.img[1]}], got {tuple(x.shape)} {x.dtype}")
-        with _dev_ctx(self.dev):
-            ver = _version(self.bb) + (_version(self.heads) if self.heads is not None else 0)
-            if ver != self.version:          # parameters changed in place: re-pack (same shapes), re-capture
-                self._pack()
-                self.graph = None
-            if not graph:
-                self._launch(x.contiguous())
-                return dict(self.out)
-            if self.static_in is None:
-                self.static_in = torch.empty_like(x, memory_format=torch.contiguous_format)
-            self.static_in.copy_(x, non_blocking=True)
-            if self.graph is None:
-                self._launch(self.static_in)  # warm-up outside capture (sets kernel attributes, loads modules)
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    self._launch(self.static_in)
-                self.graph = g
-            self.graph.replay()
-            return dict(self.out)
-
-    def launches_per_forward(self):
-        with _dev_ctx(self.dev):
-            n0 = ops.launch_count()
-            self._launch(self.static_in if self.static_in is not None else
-                         torch.zeros(self.B, 3, *self.img, device=self.dev))
-            return ops.launch_count() - n0
 
 
 # --------------------------------------------------------------------------------------------

@@ -12,8 +12,8 @@ TaskPrompter/models/transformers/taskprompter_swin.py (TP below), so reference c
                                       multi_scale_fuse, layers, norm
 used through taskprompter.TaskPrompterWrapper (models/taskprompter_wrapper.py:9-40) with ConvHead / DEConvHead.
 
-The modules own parameters; the forward is `_SwinPlan`: packed weights + a fixed workspace + one launch sequence, captured
-in a CUDA graph. What runs where:
+The modules own parameters; the forward is `_SwinPlan` (plans.Plan): packed weights + a fixed workspace + one launch
+sequence, captured in a CUDA graph. What runs where:
   * every Linear / 1x1 / 3x3 convolution on the wgmma GEMM (mtt_gemm, the named block operators);
   * window partition with cyclic shift and zero padding, with the T task prompts replicated in front of every window:
     one gather kernel writing the joint window stream [B * nW * (T + ws^2), C] (TP:326-340, :177-181);
@@ -39,8 +39,9 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .taskprompter import (PARITY, Mlp, PatchEmbed, _cached, _dev_ctx, _f32, _HeadSpace, _launch_head, _pack_head,
-                           _Streams, _trunc_normal_, _version)
+from .plans import Plan, _cached, _dev_ctx, _f32, _lin, _pack_stem
+from .taskprompter import (PARITY, Mlp, PatchEmbed, _HeadSpace, _launch_head, _pack_fuse, _pack_head,
+                           _trunc_normal_)
 
 STRIDES = (8, 16, 32, 32)          # utils/common_config.py:37: level il lives at 1/STRIDES[il] of the image
 
@@ -210,12 +211,6 @@ class TaskPrompterSwin(nn.Module):
 # --------------------------------------------------------------------------------------------
 # packed weights
 # --------------------------------------------------------------------------------------------
-def _lin(mod, device, ns):
-    w = ops.pack_weight(_f32(mod.weight, device).reshape(mod.weight.shape[0], -1), ns)
-    b = _f32(mod.bias, device) if mod.bias is not None else None
-    return w, b
-
-
 def _pack_swin_block(blk, device, ns):
     def build():
         f = lambda t: _f32(t, device)
@@ -258,29 +253,10 @@ def _pack_merge(dsm, device, ns):
 
 def _pack_swin_decoder(bb, tasks, device, ns):
     def build():
-        f = lambda t: _f32(t, device)
-        p = bb.p
-        Lv, ff = p.level_embed_dim, p.final_embed_dim
-        Lv_pad = ops.round_up(Lv, 8)
-        W = SimpleNamespace(levels=[], msf=[])
-        for il in range(bb.num_layers):
-            lv = []
-            for t in tasks:
-                tw = SimpleNamespace()
-                tw.spa, tw.spa_b = _lin(bb.fea_decode_spa[il][t][0], device, ns)
-                tw.chan, tw.chan_b = _lin(bb.fea_decode_chan[il][t][0], device, ns)
-                fu = bb.fea_fuse[il][t]
-                w0 = f(fu[0].weight).reshape(ff, 2 * Lv)
-                w0p = torch.zeros(ff, 2 * Lv_pad, device=device)      # K laid out like the `cat` buffer
-                w0p[:, :Lv] = w0[:, :Lv]
-                w0p[:, Lv_pad:Lv_pad + Lv] = w0[:, Lv:]
-                tw.f0, tw.f0_b = ops.pack_weight(w0p, ns), f(fu[0].bias)
-                tw.f1, tw.f1_b = ops.pack_conv_weight(f(fu[1].weight), fu[1].bias, fu[2], ns)   # conv3x3 + eval BN
-                tw.f4, tw.f4_b = ops.pack_conv_weight(f(fu[4].weight), fu[4].bias, None, ns)    # 3x3 here (TP:630)
-                lv.append(tw)
-            W.levels.append(lv)
-        for t in tasks:
-            W.msf.append(ops.pack_conv_weight(f(bb.multi_scale_fuse[t].weight), bb.multi_scale_fuse[t].bias, None, ns))
+        W = SimpleNamespace()
+        W.levels = [[_pack_fuse(bb, il, t, device, ns) for t in tasks] for il in range(bb.num_layers)]
+        W.msf = [ops.pack_conv_weight(_f32(bb.multi_scale_fuse[t].weight, device), bb.multi_scale_fuse[t].bias, None, ns)
+                 for t in tasks]
         return W
     return _cached(bb, ("decoder", device, ns, tuple(tasks)), build)
 
@@ -288,14 +264,15 @@ def _pack_swin_decoder(bb, tasks, device, ns):
 # --------------------------------------------------------------------------------------------
 # the fused forward
 # --------------------------------------------------------------------------------------------
-class _SwinPlan:
+class _SwinPlan(Plan):
+    """Geometry, workspace and launch sequence of one TaskPrompterSwin wrapper forward."""
+
     def __init__(self, bb, heads, tasks, target, B, device, nsplit, mode="full"):
-        ops._L.check(ops._L.load().mtt_device_check(), "mtt_device_check")
+        super().__init__((bb, heads), B, device, nsplit, max(len(tasks), 2))
         if mode not in ("full",):
             raise NotImplementedError("mtt_b200 TaskPrompterSwin: only the wrapper forward is built (no predict())")
-        device = torch.device(device)
-        self.bb, self.heads, self.tasks, self.target = bb, heads, list(tasks), target
-        self.B, self.dev, self.ns, self.mode = B, device, nsplit, mode
+        device = self.dev
+        self.bb, self.heads, self.tasks, self.target, self.mode = bb, heads, list(tasks), target, mode
         self.T = T = len(self.tasks)
         p = bb.p
         self.ce = ce = p.chan_embed_dim
@@ -304,15 +281,13 @@ class _SwinPlan:
         assert self.r * self.r == ce and self.r % self.nh == 0
         self.Lv, self.f = p.level_embed_dim, p.final_embed_dim
         self.Lv_pad, self.f_ld = ops.round_up(self.Lv, 8), ops.round_up(self.f, 8)
-        self.img = bb.full_img_size
+        self.img, self.in_chans = bb.full_img_size, bb.in_chans
         self.ds_img = tuple(bb.patch_embed.img_size)
-        self.graph, self.static_in = None, None
-        self.streams = _Streams(device, max(T, 2))
         ns = nsplit
         S = lambda r, c, **kw: ops.Split(r, c, device, ns, **kw)
         z = lambda *s: torch.zeros(*s, device=device, dtype=torch.float32)
         with _dev_ctx(device):
-            self._pack()
+            self._repack()
             E, patch = bb.embed_dim, bb.patch_size
             gh, gw = bb.patch_grid
             self.img_ds = z(B, bb.in_chans, *self.ds_img) if self.ds_img != self.img else None
@@ -390,30 +365,11 @@ class _SwinPlan:
 
     def _pack(self):
         bb, dev, ns = self.bb, self.dev, self.ns
-        f = lambda t: _f32(t, dev)
-
-        def stem():
-            W = SimpleNamespace()
-            W.pe_w = ops.pack_weight(f(bb.patch_embed.proj.weight).reshape(bb.embed_dim, -1), ns)
-            W.pe_b = f(bb.patch_embed.proj.bias)
-            W.pnw, W.pnb, W.pneps = f(bb.patch_embed.norm.weight), f(bb.patch_embed.norm.bias), bb.patch_embed.norm.eps
-            W.prompts = f(bb.task_prompts)
-            W.nw, W.nb, W.neps = f(bb.norm.weight), f(bb.norm.bias), bb.norm.eps
-            return W
-        self.Ws = _cached(bb, ("stem", dev, ns), stem)
+        self.Ws = _pack_stem(bb, dev, ns)
         self.Wb = [[_pack_swin_block(blk, dev, ns) for blk in layer.blocks] for layer in bb.layers]
         self.Wm = [_pack_merge(layer.downsample, dev, ns) if layer.downsample is not None else None for layer in bb.layers]
         self.Wd = _pack_swin_decoder(bb, self.tasks, dev, ns)
         self.Wh = [_pack_head(self.heads[t], dev, ns) for t in self.tasks]
-        self.version = _version(bb) + _version(self.heads)
-
-    @property
-    def serial(self):
-        return self.streams.serial
-
-    @serial.setter
-    def serial(self, v):
-        self.streams.serial = bool(v)
 
     # ------------------------------------------------------------------------------------------
     def _block(self, s, w, blk):
@@ -519,36 +475,6 @@ class _SwinPlan:
         self._level(n_stage - 1, self.xfin, last.logits, last.rc)
         self.streams.par([lambda ti=ti, t=t, hw=hw, hs=hs: self._head_chain(ti, t, hw, hs)
                           for ti, (t, hw, hs) in enumerate(zip(self.tasks, self.Wh, self.hs))])
-
-    def run(self, x, graph=True):
-        if tuple(x.shape[1:]) != (self.bb.in_chans, *self.img) or x.dtype != torch.float32:
-            raise ValueError(f"expected fp32 input [B,3,{self.img[0]},{self.img[1]}], got {tuple(x.shape)} {x.dtype}")
-        with _dev_ctx(self.dev):
-            if _version(self.bb) + _version(self.heads) != self.version:
-                self._pack()
-                self.graph = None
-            if not graph:
-                self._launch(x.contiguous())
-                return dict(self.out)
-            if self.static_in is None:
-                self.static_in = torch.empty_like(x, memory_format=torch.contiguous_format)
-            self.static_in.copy_(x, non_blocking=True)
-            if self.graph is None:
-                self._launch(self.static_in)
-                torch.cuda.synchronize()
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    self._launch(self.static_in)
-                self.graph = g
-            self.graph.replay()
-            return dict(self.out)
-
-    def launches_per_forward(self):
-        with _dev_ctx(self.dev):
-            n0 = ops.launch_count()
-            self._launch(self.static_in if self.static_in is not None else
-                         torch.zeros(self.B, 3, *self.img, device=self.dev))
-            return ops.launch_count() - n0
 
 
 def build_from_config(cfg, nsplit=PARITY, use_graph=True):

@@ -140,6 +140,21 @@ def test_invpt_rejects_the_sizes_the_reference_rejects(monkeypatch):
         model.plan(1, torch.device("cpu"))
 
 
+def test_invpt_predict_refuses_a_task_without_post_processing(monkeypatch):
+    """predict() fuses the reference's get_output into the final resize; a task get_output defines nothing for is
+    refused when the plan is built, with the ValueError TaskPrompter's predict() raises."""
+    import mtt_b200  # noqa: F401
+    from mtt_b200 import invpt as IP
+    import emul_ops
+
+    emul_ops.install(monkeypatch)
+    cfg = dict(tasks=["semseg", "3ddet"], num_output={"semseg": 5, "3ddet": 1}, img_size=(64, 64), patch=16, C=128,
+               depth=4, heads=2, select=[1, 2, 3], embed_dim=32, pred_const=16, down=2, name="ip_3ddet")
+    model = IP.build_from_config(cfg, nsplit=2, use_graph=False).eval()
+    with pytest.raises(ValueError, match="no get_output post-processing defined for task '3ddet'"):
+        model.plan(1, torch.device("cpu"), postproc=True)
+
+
 # ---- error behaviour and odd-but-legal arguments -----------------------------------------------------------------------
 _TP_BASE = dict(tasks=["semseg", "depth"], num_output={"semseg": 5, "depth": 1}, img_size=(64, 64), patch=16, C=128, depth=4,
                 heads=2, select=[1, 2, 3], e=24, f=32, use_ctr=True, chan_nheads=1, name="edge", prompt_len=1, head="conv")
