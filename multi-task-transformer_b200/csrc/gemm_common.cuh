@@ -129,20 +129,46 @@ __device__ __forceinline__ RowInfo row_info(const GemmParams& p, int ms, int row
 }
 
 // ---- fused epilogue for the two adjacent accumulator columns n, n + 1 of one row (the pair a thread holds in the
-// wgmma accumulator fragment): bias, activation, residual, fp32 and split-bf16 stores
-__device__ __forceinline__ void epilogue_store2(const GemmParams& p, float v0, float v1, int n, const RowInfo& ri) {
-  if (n >= p.N) return;
+// wgmma accumulator fragment): bias, activation, residual, fp32 and split-bf16 stores.
+// The global reads (bias, residual) of a batch of pairs are issued by epilogue_load2 before any of the batch's stores:
+// the residual may be the output itself (x += f(x)), so the compiler cannot move a read above an earlier store, and
+// one read at a time would wait out the full memory latency for each. Every element is read and written by one
+// thread only, so reading a batch first is safe.
+struct EpiIn {
+  float2 b, r;  // bias and residual of the pair (zero where absent)
+};
+__device__ __forceinline__ EpiIn epilogue_load2(const GemmParams& p, int n, const RowInfo& ri) {
+  EpiIn e{make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+  if (n >= p.N) return e;
   const bool two = n + 1 < p.N;
   const bool vec = two && p.vec_ok;  // n is even: 8-byte fp32 pairs and 4-byte bf16 pairs are aligned
   if (p.bias) {
     if (vec) {
-      const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-      v0 += b.x;
-      v1 += b.y;
+      e.b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
     } else {
-      v0 += __ldg(p.bias + n);
-      if (two) v1 += __ldg(p.bias + n + 1);
+      e.b.x = __ldg(p.bias + n);
+      if (two) e.b.y = __ldg(p.bias + n + 1);
     }
+  }
+  if (p.residual) {
+    const float* rp = p.residual + ri.mr * p.ldr + n;
+    if (vec) {
+      e.r = *reinterpret_cast<const float2*>(rp);
+    } else {
+      e.r.x = rp[0];
+      if (two) e.r.y = rp[1];
+    }
+  }
+  return e;
+}
+__device__ __forceinline__ void epilogue_store2(const GemmParams& p, float v0, float v1, int n, const RowInfo& ri,
+                                                const EpiIn& e) {
+  if (n >= p.N) return;
+  const bool two = n + 1 < p.N;
+  const bool vec = two && p.vec_ok;
+  if (p.bias) {
+    v0 += e.b.x;
+    v1 += e.b.y;
   }
   if (p.act == MTT_ACT_GELU) {
     v0 = gelu_erf(v0);
@@ -152,15 +178,8 @@ __device__ __forceinline__ void epilogue_store2(const GemmParams& p, float v0, f
     v1 = fmaxf(v1, 0.f);
   }
   if (p.residual) {
-    const float* rp = p.residual + ri.mr * p.ldr + n;
-    if (vec) {
-      const float2 a = *reinterpret_cast<const float2*>(rp);
-      v0 += a.x;
-      v1 += a.y;
-    } else {
-      v0 += rp[0];
-      if (two) v1 += rp[1];
-    }
+    v0 += e.r.x;
+    v1 += e.r.y;
   }
   if (p.out_f32) {
     float* op = p.out_f32 + ri.mo * p.ldo_f32 + n;

@@ -11,7 +11,7 @@
 // Tiles are 128 x BN (BN = 128, or 256 for wide problems).  Roles (384 threads): warpgroup 0 = TMA producer (one
 // warp issues, the warpgroup hands its registers to the consumers), warpgroups 1 and 2 = consumers, each owning 64
 // rows of the tile: they wait for a stage, issue the wgmma chain on it, release the stage and, after the last k-block
-// of a tile, run the fused epilogue straight from the accumulator registers.  One barrier ring (smem full / empty)
+// of a tile, run the fused epilogue through a per-warp shared-memory buffer.  One barrier ring (smem full / empty)
 // and a static persistent tile schedule; the producer runs ahead into the next tile while the epilogue drains.
 //
 // Convolution (mode 1) is the same kernel: the A tile of 128 output pixels is a TH x TW patch of one
@@ -23,12 +23,17 @@
 
 namespace mtt {
 
+constexpr int kEpiCols = 64;  // columns per staged epilogue chunk
+
 template <int NSPLIT, int BN>
 struct GemmCfg {
   static constexpr uint32_t kBTileBytes = BN * BK * 2;
   static constexpr uint32_t kStageBytes = NSPLIT * (kTileBytes + kBTileBytes);
   static constexpr int kStages = (200 * 1024) / kStageBytes;  // 3 / 6 stages (BN 128), 2 / 4 (BN 256)
-  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 1024 + 256;
+  // stages | 256 B of mbarriers | one 16 x kEpiCols fp32 epilogue buffer per consumer warp (+ 1 KB for alignment)
+  static constexpr uint32_t kEpiBufBytes = kEpiWarps * 16 * kEpiCols * 4;
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 256 + kEpiBufBytes + 1024;
+  static_assert(kSmemBytes <= 227 * 1024, "exceeds the per-block shared memory of sm_90");
 };
 
 // ---- stream-K tail (SK = true, single-problem kernel with 256-wide tiles) ------------------------------------------------
@@ -110,6 +115,11 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
   using Cfg = GemmCfg<NSPLIT, BN>;
   constexpr int ST = Cfg::kStages;
   constexpr uint32_t kBT = Cfg::kBTileBytes;
+  // A planes whose fragments the consumers hold in registers for a stage (8 registers per k16 step and plane) and feed
+  // to RS-form wgmma. Beside the 128 x 256 tile's acc[128] + part[64] only A_hi fits without spilling; its A_lo
+  // (one wgmma per k16 step and half) stays in the shared-memory (SS) form.
+  constexpr int kRegPlanes = BN == 128 ? NSPLIT : 1;
+  constexpr uint32_t kTurnBar = 1;  // named barriers 1, 2: the consumer warpgroups' turns
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -190,10 +200,27 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
     const int row0 = cw * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's rows: row0 and row0 + 8
     const int col0 = 2 * (lane & 3);           // ... and columns col0 + 8 i + {0, 1}
     const uint32_t a_off = (uint32_t)cw * 64 * 128;
+    // ldmatrix source of this lane in the warpgroup's 64 A rows: row (lane % 8) + 8 ((lane / 8) % 2) of the warp's 16,
+    // 16-byte chunk 2 ks + lane / 16 of the 128-byte row, stored at chunk ^ (row % 8) by the 128-byte swizzle
+    const int lrow = (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+    const uint32_t a_frag_off = a_off + (uint32_t)lrow * 128;
+    const int a_chunk = lane >> 4, a_xor = lane & 7;
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];   // the tile's fp32 sum, in the m64nBN fragment layout (= the 128-column halves side by side)
     float part[64];      // one stage's products for one 128-column half
+    uint32_t afr[BK / 16][kRegPlanes][4];  // the stage's A fragments per k16 step (RS-form wgmma)
+    // Ordered consumer warpgroups: the two warpgroups take turns issuing their wgmma chains (one chain = one stage x
+    // one 128-column half), so that while one waits for its chain and folds it into acc, the other's chain keeps the
+    // tensor pipe busy. Named barrier kTurnBar + w opens warpgroup w's turn; each side arrives at the other's barrier
+    // after issuing. Warpgroup 1 opens the first turn, warpgroup 0 consumes the last opening after its loop.
+    auto wait_turn = [&] {  // barrier ids are immediates; cw is uniform per warpgroup
+      if (cw == 0) bar_sync<kTurnBar, 256>(); else bar_sync<kTurnBar + 1, 256>();
+    };
+    auto pass_turn = [&] {
+      if (cw == 0) bar_arrive<kTurnBar + 1, 256>(); else bar_arrive<kTurnBar, 256>();
+    };
+    if (cw == 1) pass_turn();
     for (int si = 0; si < sched.n_seg; ++si) {
       int tile, kbeg, kend;
       sk_piece(sched, si, k_iters, tile, kbeg, kend);
@@ -209,30 +236,47 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
         if (kb == p.num_kb) kb = 0;
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint32_t a_hi = sa + a_off, a_lo = sa + kTileBytes + a_off;
+        const uint32_t a_lo = sa + kTileBytes + a_off;
         const uint32_t b_hi = sa + NSPLIT * kTileBytes, b_lo = b_hi + kBT;
+        {  // each A fragment in registers is read from shared memory once per stage, not once per wgmma using it
+          const uint32_t fa = sa + a_frag_off;
+#pragma unroll
+          for (int ks = 0; ks < BK / 16; ++ks) {
+            const uint32_t sw = (uint32_t)(((2 * ks + a_chunk) ^ a_xor) << 4);
+#pragma unroll
+            for (int s = 0; s < kRegPlanes; ++s) ldmatrix_x4(afr[ks][s], fa + s * kTileBytes + sw);
+          }
+        }
         // The tensor core adds products into its accumulator with truncation, so a long chain of wgmma on one
         // accumulator drifts towards zero (a one-sided error that grows with K). Each stage's products are therefore
         // summed in a fresh accumulator and added to the tile's sum with a round-to-nearest FADD.
 #pragma unroll
         for (int hn = 0; hn < BN / 128; ++hn) {
           const uint32_t bo = (uint32_t)hn * 128 * 128;  // 128 weight rows of 128 bytes
+          wait_turn();
           wgmma_fence_regs(part);
           wgmma_fence();
 #pragma unroll
           for (int ks = 0; ks < BK / 16; ++ks) {
             if (ks >= nks) break;
-            const uint64_t adh = gmma_desc_sw128(a_hi + ks * 32);
             const uint64_t bdh = gmma_desc_sw128(b_hi + bo + ks * 32);
-            wgmma_ss_n128<0>(part, adh, bdh, ks > 0 ? 1 : 0);
+            wgmma_rs_n128<0>(part, afr[ks][0], bdh, ks > 0 ? 1 : 0);
             if (NSPLIT == 2) {
-              wgmma_ss_n128<0>(part, adh, gmma_desc_sw128(b_lo + bo + ks * 32), 1);
-              wgmma_ss_n128<0>(part, gmma_desc_sw128(a_lo + ks * 32), bdh, 1);
+              wgmma_rs_n128<0>(part, afr[ks][0], gmma_desc_sw128(b_lo + bo + ks * 32), 1);
+              if (kRegPlanes == 2)
+                wgmma_rs_n128<0>(part, afr[ks][1], bdh, 1);
+              else
+                wgmma_ss_n128<0>(part, gmma_desc_sw128(a_lo + ks * 32), bdh, 1);
             }
           }
           wgmma_commit();
+          pass_turn();
           wgmma_wait<0>();
           wgmma_fence_regs(part);
+#pragma unroll
+          for (int ks = 0; ks < BK / 16; ++ks)
+#pragma unroll
+            for (int s = 0; s < kRegPlanes; ++s) wgmma_fence_regs(afr[ks][s]);
 #pragma unroll
           for (int i = 0; i < 64; ++i) acc[hn * 64 + i] += part[i];
         }
@@ -286,24 +330,58 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
         }
       }
       if (p.debug & 2) continue;
-      GemmParams pq = p;                      // grouped: this problem's pointers over the shared geometry
+      GemmParams pg;                          // grouped: this problem's pointers over the shared geometry
       if (GROUPED) {
+        pg = p;
         const GroupProblem& gp = grp->prob[g];
-        pq.bias = gp.bias;
-        pq.residual = gp.residual;
-        pq.out_f32 = gp.out_f32;
-        pq.out_hi = gp.out_hi;
-        pq.out_lo = gp.out_lo;
+        pg.bias = gp.bias;
+        pg.residual = gp.residual;
+        pg.out_f32 = gp.out_f32;
+        pg.out_hi = gp.out_hi;
+        pg.out_lo = gp.out_lo;
       }
+      const GemmParams& pq = GROUPED ? pg : p;  // single problem: read straight from the kernel parameters
+      // The warp's 16 x BN slice goes out in 16 x kEpiCols chunks through its shared-memory buffer: the fragment is
+      // written with one unrolled store per column pair (acc needs compile-time indices), and a rolled loop over rows
+      // then runs the epilogue with lane l on columns 2 l, 2 l + 1, so each row is one contiguous warp-wide store.
+      // Unrolling the epilogue itself over the fragment made it tens of thousands of instructions long and bound by
+      // instruction fetch. Columns are XOR-swizzled by row in 8-column groups, so both sides are free of bank conflicts.
+      const int wrow0 = cw * 64 + (warp & 3) * 16;  // the warp's first row in the tile
+      float* ebuf = reinterpret_cast<float*>(smem + ST * Cfg::kStageBytes + 256) + ew * 16 * kEpiCols;
+      // rows whose bias / residual reads are in flight together; more spills beside the 128 x 256 tile's acc[128]
+      constexpr int kEpiRows = BN == 128 ? 8 : 1;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const RowInfo ri = row_info(p, mt, row0 + 8 * h);
-        if (!ri.ok) continue;
+      for (int c0 = 0; c0 < BN; c0 += kEpiCols) {
 #pragma unroll
-        for (int i = 0; i < BN / 8; ++i)
-          epilogue_store2(pq, acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1], nt * BN + 8 * i + col0, ri);
+        for (int j = 0; j < kEpiCols / 8; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = (lane >> 2) + 8 * h, i = c0 / 8 + j;
+            *reinterpret_cast<float2*>(ebuf + r * kEpiCols + ((8 * j + col0) ^ ((r & 7) << 3))) =
+                make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+          }
+        __syncwarp();
+        const int n = nt * BN + c0 + 2 * lane;
+#pragma unroll 1
+        for (int r0 = 0; r0 < 16; r0 += kEpiRows) {
+          RowInfo ri[kEpiRows];
+          EpiIn in[kEpiRows] = {};  // this batch's bias / residual reads are issued before its stores
+#pragma unroll
+          for (int k = 0; k < kEpiRows; ++k) {
+            ri[k] = row_info(p, mt, wrow0 + r0 + k);
+            if (ri[k].ok) in[k] = epilogue_load2(pq, n, ri[k]);
+          }
+#pragma unroll
+          for (int k = 0; k < kEpiRows; ++k) {
+            const int r = r0 + k;
+            const float2 v = *reinterpret_cast<const float2*>(ebuf + r * kEpiCols + ((2 * lane) ^ ((r & 7) << 3)));
+            if (ri[k].ok) epilogue_store2(pq, v.x, v.y, n, ri[k], in[k]);
+          }
+        }
+        __syncwarp();
       }
     }
+    if (cw == 0) wait_turn();  // warpgroup 1's last opening: both barriers end their last phase
   }
 }
 
