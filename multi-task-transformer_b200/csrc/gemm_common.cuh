@@ -36,7 +36,8 @@ struct GemmParams {
   int vec_ok;
   int vec32_ok;  // every epilogue pointer / stride allows 32-byte accesses
   int a_groups_per_tile;  // >0: A rows are gathered in groups through a rank-3 tensor map
-  int debug;              // profiling aid (env MTT_GEMM_DEBUG): bit0 = skip TMA loads, bit1 = skip global stores
+  int debug;              // profiling aid (env MTT_GEMM_DEBUG): bit0 = skip TMA loads, bit1 = skip the epilogue,
+                          // bit2 = run the epilogue without its global stores
   // stream-K tail of the 128 x 256 kernel: the first sk_tiles tiles are split along K over ALL CTAs
   int sk_tiles;           // 0: every tile is computed by one CTA
   float* sk_part;         // [CTA][128 rows][256 columns] fp32 partial accumulators
@@ -128,47 +129,29 @@ __device__ __forceinline__ RowInfo row_info(const GemmParams& p, int ms, int row
   return r;
 }
 
-// ---- fused epilogue for the two adjacent accumulator columns n, n + 1 of one row (the pair a thread holds in the
-// wgmma accumulator fragment): bias, activation, residual, fp32 and split-bf16 stores.
-// The global reads (bias, residual) of a batch of pairs are issued by epilogue_load2 before any of the batch's stores:
-// the residual may be the output itself (x += f(x)), so the compiler cannot move a read above an earlier store, and
-// one read at a time would wait out the full memory latency for each. Every element is read and written by one
-// thread only, so reading a batch first is safe.
-struct EpiIn {
-  float2 b, r;  // bias and residual of the pair (zero where absent)
-};
-__device__ __forceinline__ EpiIn epilogue_load2(const GemmParams& p, int n, const RowInfo& ri) {
-  EpiIn e{make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-  if (n >= p.N) return e;
+// ---- fused epilogue for the two adjacent columns n, n + 1 of one row: bias, activation, residual, fp32 and
+// split-bf16 stores. The kernel reads the bias (epilogue_bias2) and the residual (staged in shared memory) before it
+// calls epilogue_store2, which only computes and stores.
+__device__ __forceinline__ float2 epilogue_bias2(const GemmParams& p, int n) {  // zero where absent or n >= N
+  float2 b = make_float2(0.f, 0.f);
+  if (!p.bias || n >= p.N) return b;
+  if (n + 1 < p.N && p.vec_ok) {  // n is even: 8-byte fp32 pairs are aligned
+    b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+  } else {
+    b.x = __ldg(p.bias + n);
+    if (n + 1 < p.N) b.y = __ldg(p.bias + n + 1);
+  }
+  return b;
+}
+// mo: output row (RowInfo::mo); b, r: bias and residual of the pair
+__device__ __forceinline__ void epilogue_store2(const GemmParams& p, float v0, float v1, int n, long long mo, float2 b,
+                                                float2 r) {
+  if (n >= p.N) return;
   const bool two = n + 1 < p.N;
   const bool vec = two && p.vec_ok;  // n is even: 8-byte fp32 pairs and 4-byte bf16 pairs are aligned
   if (p.bias) {
-    if (vec) {
-      e.b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-    } else {
-      e.b.x = __ldg(p.bias + n);
-      if (two) e.b.y = __ldg(p.bias + n + 1);
-    }
-  }
-  if (p.residual) {
-    const float* rp = p.residual + ri.mr * p.ldr + n;
-    if (vec) {
-      e.r = *reinterpret_cast<const float2*>(rp);
-    } else {
-      e.r.x = rp[0];
-      if (two) e.r.y = rp[1];
-    }
-  }
-  return e;
-}
-__device__ __forceinline__ void epilogue_store2(const GemmParams& p, float v0, float v1, int n, const RowInfo& ri,
-                                                const EpiIn& e) {
-  if (n >= p.N) return;
-  const bool two = n + 1 < p.N;
-  const bool vec = two && p.vec_ok;
-  if (p.bias) {
-    v0 += e.b.x;
-    v1 += e.b.y;
+    v0 += b.x;
+    v1 += b.y;
   }
   if (p.act == MTT_ACT_GELU) {
     v0 = gelu_erf(v0);
@@ -178,11 +161,15 @@ __device__ __forceinline__ void epilogue_store2(const GemmParams& p, float v0, f
     v1 = fmaxf(v1, 0.f);
   }
   if (p.residual) {
-    v0 += e.r.x;
-    v1 += e.r.y;
+    v0 += r.x;
+    v1 += r.y;
+  }
+  if (p.debug & 4) {  // profiling aid: the arithmetic runs, the global stores do not
+    asm volatile("" ::"f"(v0), "f"(v1));
+    return;
   }
   if (p.out_f32) {
-    float* op = p.out_f32 + ri.mo * p.ldo_f32 + n;
+    float* op = p.out_f32 + mo * p.ldo_f32 + n;
     if (vec) {
       *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
     } else {
@@ -191,7 +178,7 @@ __device__ __forceinline__ void epilogue_store2(const GemmParams& p, float v0, f
     }
   }
   if (p.out_hi) {
-    const long long o = ri.mo * p.ldo_bf + n;
+    const long long o = mo * p.ldo_bf + n;
     if (vec) {
       uint32_t h, l;
       split_pack2(v0, v1, h, l);

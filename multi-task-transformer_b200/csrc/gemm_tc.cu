@@ -23,16 +23,18 @@
 
 namespace mtt {
 
-constexpr int kEpiCols = 64;  // columns per staged epilogue chunk
+constexpr int kEpiCols = 32;  // columns per staged epilogue chunk: 16 lanes per row, two rows per pass
 
 template <int NSPLIT, int BN>
 struct GemmCfg {
   static constexpr uint32_t kBTileBytes = BN * BK * 2;
   static constexpr uint32_t kStageBytes = NSPLIT * (kTileBytes + kBTileBytes);
   static constexpr int kStages = (200 * 1024) / kStageBytes;  // 3 / 6 stages (BN 128), 2 / 4 (BN 256)
-  // stages | 256 B of mbarriers | one 16 x kEpiCols fp32 epilogue buffer per consumer warp (+ 1 KB for alignment)
-  static constexpr uint32_t kEpiBufBytes = kEpiWarps * 16 * kEpiCols * 4;
-  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 256 + kEpiBufBytes + 1024;
+  // stages | 256 B of mbarriers | per consumer warp, a 16 x kEpiCols fp32 accumulator chunk and the residual of that
+  // chunk | per consumer warp, the residual-row table (+ 1 KB for alignment)
+  static constexpr uint32_t kEpiBufBytes = kEpiWarps * 2 * 16 * kEpiCols * 4;
+  static constexpr uint32_t kRowMapBytes = kEpiWarps * 16 * 8;  // per consumer warp, the residual rows of its 16 rows
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 256 + kEpiBufBytes + kRowMapBytes + 1024;
   static_assert(kSmemBytes <= 227 * 1024, "exceeds the per-block shared memory of sm_90");
 };
 
@@ -205,6 +207,36 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
     const int lrow = (warp & 3) * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
     const uint32_t a_frag_off = a_off + (uint32_t)lrow * 128;
     const int a_chunk = lane >> 4, a_xor = lane & 7;
+    const int wrow0 = cw * 64 + (warp & 3) * 16;  // the warp's first row in the tile
+    float* ebuf = reinterpret_cast<float*>(smem + ST * Cfg::kStageBytes + 256) + ew * 2 * 16 * kEpiCols;
+    float* rbuf = ebuf + 16 * kEpiCols;  // the residual of the chunk in ebuf
+    // the residual row of each of the warp's 16 rows (-1: the row is not written), set when a piece starts; kept in
+    // shared memory, since the registers beside the 128 x 256 tile's accumulator are few
+    long long* rmap = reinterpret_cast<long long*>(smem + ST * Cfg::kStageBytes + 256 + Cfg::kEpiBufBytes) + ew * 16;
+    // Copies the residual of rows [8 half, 8 half + 8) of the warp's 16, columns [n0, n0 + kEpiCols), to rbuf as one
+    // cp.async group. Lane l copies columns 4 (l % 8) .. 4 (l % 8) + 3 of rows 8 half + l / 8 and 8 half + l / 8 + 4;
+    // what lies outside the problem is zero-filled.
+    auto res_issue = [&](const float* res, int n0, int half) {
+      const int n = n0 + 4 * (lane & 7);
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const int r = 8 * half + (lane >> 3) + 4 * k;
+        const long long m = rmap[r];
+        const uint32_t dst = smem_u32(rbuf + r * kEpiCols + 4 * (lane & 7));
+        const float* src = res + (m >= 0 ? m * p.ldr + n : 0);
+        if (p.vec_ok) {  // residual and ldr 16-byte aligned, n % 4 == 0
+          const int cols = m >= 0 ? min(max(p.N - n, 0), 4) : 0;
+          cp_async_cg16(dst, cols ? src : res, 4 * cols);
+        } else {
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const bool in = m >= 0 && n + e < p.N;
+            cp_async_ca4(dst + 4 * e, in ? src + e : res, in ? 4 : 0);
+          }
+        }
+      }
+      cp_async_commit();
+    };
     int stage = 0;
     uint32_t phase = 0;
     float acc[BN / 2];   // the tile's fp32 sum, in the m64nBN fragment layout (= the 128-column halves side by side)
@@ -228,6 +260,19 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
       const int tl = GROUPED ? tile - g * tpp : tile;
       const int mt = tl % p.tiles_m;
       const int nt = tl / p.tiles_m;
+      {  // the residual of the epilogue's first chunk: the copy has the whole mainloop to land, and is issued while acc
+         // holds nothing (rbuf is free: the previous piece's epilogue has read it)
+        const float* res = GROUPED ? grp->prob[g].residual : p.residual;
+        if (res && !(SK && kbeg > 0) && !(p.debug & 2)) {  // a stream-K contribution has no epilogue
+          if (lane < 16) {
+            const RowInfo ri = row_info(p, mt, wrow0 + lane);
+            rmap[lane] = ri.ok ? ri.mr : -1;
+          }
+          __syncwarp();
+          res_issue(res, nt * BN, 0);
+          res_issue(res, nt * BN, 1);
+        }
+      }
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       int kb = kbeg % p.num_kb;
@@ -341,44 +386,73 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
         pg.out_lo = gp.out_lo;
       }
       const GemmParams& pq = GROUPED ? pg : p;  // single problem: read straight from the kernel parameters
-      // The warp's 16 x BN slice goes out in 16 x kEpiCols chunks through its shared-memory buffer: the fragment is
-      // written with one unrolled store per column pair (acc needs compile-time indices), and a rolled loop over rows
-      // then runs the epilogue with lane l on columns 2 l, 2 l + 1, so each row is one contiguous warp-wide store.
-      // Unrolling the epilogue itself over the fragment made it tens of thousands of instructions long and bound by
-      // instruction fetch. Columns are XOR-swizzled by row in 8-column groups, so both sides are free of bank conflicts.
-      const int wrow0 = cw * 64 + (warp & 3) * 16;  // the warp's first row in the tile
-      float* ebuf = reinterpret_cast<float*>(smem + ST * Cfg::kStageBytes + 256) + ew * 16 * kEpiCols;
-      // rows whose bias / residual reads are in flight together; more spills beside the 128 x 256 tile's acc[128]
-      constexpr int kEpiRows = BN == 128 ? 8 : 1;
-#pragma unroll
-      for (int c0 = 0; c0 < BN; c0 += kEpiCols) {
-#pragma unroll
-        for (int j = 0; j < kEpiCols / 8; ++j)
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const int r = (lane >> 2) + 8 * h, i = c0 / 8 + j;
-            *reinterpret_cast<float2*>(ebuf + r * kEpiCols + ((8 * j + col0) ^ ((r & 7) << 3))) =
-                make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
-          }
-        __syncwarp();
-        const int n = nt * BN + c0 + 2 * lane;
+      // The warp's 16 x BN slice goes out in 16 x kEpiCols chunks through its shared-memory buffer, with no global
+      // load on the per-row path:
+      //   * row map: lane l holds the output row of the warp's row l % 16 (row_info, once per piece), which the row
+      //     loop reads with a shuffle; the residual rows are in rmap;
+      //   * the bias pair is read once per chunk, while the fragment is written to ebuf;
+      //   * the chunk's residual is in rbuf (cp.async: the first chunk's was issued when the piece started, each half
+      //     of a later chunk's while the same half of the chunk before it is stored).
+      // The fragment is written with unrolled stores (acc needs compile-time indices, hence the branch per chunk in
+      // the rolled chunk loop), then 8 passes store two rows each, lanes 0-15 on row 2 q and 16-31 on row 2 q + 1, two
+      // columns per lane, one contiguous 128-byte fp32 segment per row. Unrolling the whole epilogue over the fragment
+      // made it tens of thousands of instructions long and bound by instruction fetch. Columns are XOR-swizzled by row
+      // in 8-column groups, so both sides of ebuf are free of bank conflicts.
+      // The residual may be the output itself (x += f(x)): a chunk's residual is in shared memory before any store of
+      // that chunk, and the copy of chunk c + 1 overlaps only the stores of chunk c, whose columns are disjoint from it.
+      long long mo_map;
+      {
+        const RowInfo ri = row_info(p, mt, wrow0 + (lane & 15));
+        mo_map = ri.ok ? ri.mo : -1;
+      }
+      const int hr = lane >> 4, cl = 2 * (lane & 15);  // this lane's row in a pass (2 q + hr) and column in a chunk
+      constexpr int kChunks = BN / kEpiCols;
 #pragma unroll 1
-        for (int r0 = 0; r0 < 16; r0 += kEpiRows) {
-          RowInfo ri[kEpiRows];
-          EpiIn in[kEpiRows] = {};  // this batch's bias / residual reads are issued before its stores
+      for (int c = 0; c < kChunks; ++c) {
+        const int n0 = nt * BN + c * kEpiCols, n = n0 + cl;
+        const float2 b = epilogue_bias2(pq, n);
 #pragma unroll
-          for (int k = 0; k < kEpiRows; ++k) {
-            ri[k] = row_info(p, mt, wrow0 + r0 + k);
-            if (ri[k].ok) in[k] = epilogue_load2(pq, n, ri[k]);
-          }
+        for (int cc = 0; cc < kChunks; ++cc) {
+          if (cc != c) continue;
 #pragma unroll
-          for (int k = 0; k < kEpiRows; ++k) {
-            const int r = r0 + k;
-            const float2 v = *reinterpret_cast<const float2*>(ebuf + r * kEpiCols + ((2 * lane) ^ ((r & 7) << 3)));
-            if (ri[k].ok) epilogue_store2(pq, v.x, v.y, n, ri[k], in[k]);
-          }
+          for (int j = 0; j < kEpiCols / 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int r = (lane >> 2) + 8 * h, i = cc * (kEpiCols / 8) + j;
+              *reinterpret_cast<float2*>(ebuf + r * kEpiCols + ((8 * j + col0) ^ ((r & 3) << 3))) =
+                  make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+            }
         }
+        // rows [8 half, 8 half + 8) of the chunk: 4 passes
+        auto store_rows = [&](int half) {
+#pragma unroll
+          for (int q = 4 * half; q < 4 * half + 4; ++q) {
+            const int r = 2 * q + hr;
+            const long long mo = __shfl_sync(0xffffffffu, mo_map, r);
+            const float2 v = *reinterpret_cast<const float2*>(ebuf + r * kEpiCols + (cl ^ ((r & 3) << 3)));
+            const float2 rv = pq.residual ? *reinterpret_cast<const float2*>(rbuf + r * kEpiCols + cl)
+                                          : make_float2(0.f, 0.f);
+            if (mo >= 0) epilogue_store2(pq, v.x, v.y, n, mo, b, rv);
+          }
+        };
+        // The residual arrives in two groups per chunk, rows 0-7 and rows 8-15; each half of rbuf is refilled with the
+        // next chunk's rows as soon as this chunk's passes over it are done.
+        if (pq.residual) cp_async_wait<1>();
         __syncwarp();
+        store_rows(0);
+        if (pq.residual) {
+          __syncwarp();
+          if (c + 1 < kChunks) {
+            res_issue(pq.residual, n0 + kEpiCols, 0);
+            cp_async_wait<1>();
+          } else {
+            cp_async_wait<0>();
+          }
+          __syncwarp();
+        }
+        store_rows(1);
+        __syncwarp();  // ebuf and rbuf are free for the next chunk
+        if (pq.residual && c + 1 < kChunks) res_issue(pq.residual, n0 + kEpiCols, 1);
       }
     }
     if (cw == 0) wait_turn();  // warpgroup 1's last opening: both barriers end their last phase

@@ -138,6 +138,23 @@ __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.b
 // ... and have completed their global writes (before the CTA exits)
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
+// ---------------------------------------------------------------- cp.async (per-thread asynchronous copy)
+// global -> shared copy of 16 (.cg: through L2 only) or 4 bytes, of which the first src_bytes are read and the rest
+// zero-filled (src_bytes = 0 reads nothing). Completion: cp_async_commit closes this thread's group, cp_async_wait<n>
+// waits until at most the n most recent of its groups are pending; other threads see the data after a barrier
+// (__syncwarp within a warp).
+__device__ __forceinline__ void cp_async_cg16(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_ca4(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(kPending) : "memory");
+}
+
 // L2 prefetch of a tensor-map box (no shared-memory destination, no barrier)
 __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* m, int c0, int c1) {
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(m)),

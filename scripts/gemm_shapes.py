@@ -8,12 +8,14 @@ launch reports M summed over its problems, a 3x3 convolution K x 9. Enough forwa
 at least --min-launches launches after --warmup forwards. One torch.profiler pass over a single forward names the
 kernel instantiation (tile width, grouped or not) and grid of every launch.
 
-Run three times, each in its own process because the library reads MTT_GEMM_DEBUG once:
+Run four times, each in its own process because the library reads MTT_GEMM_DEBUG once:
   full           the kernel as shipped;
   no_loads       MTT_GEMM_DEBUG=1: the producer issues no TMA loads (the consumers compute on stale shared memory);
-  no_epilogue    MTT_GEMM_DEBUG=2: no global stores after the mainloop.
+  no_epilogue    MTT_GEMM_DEBUG=2: no epilogue after the mainloop (no bias / residual reads, no stores);
+  no_stores      MTT_GEMM_DEBUG=4: the whole epilogue except its global stores.
 Only the timings of the debug runs are used, never their outputs. full - no_loads approximates the operand delivery
-cost, full - no_epilogue the epilogue cost; what no_loads leaves is MMA + fold (+ epilogue).
+cost, full - no_epilogue the epilogue cost, and full - no_stores the part of it that is store drain; what no_loads
+leaves is MMA + fold (+ epilogue).
 
 Prints one JSON line per (run, shape), then one summary line per run. Needs a GPU; reads the card's name, power limit
 and SM clock with nvidia-smi in the same call.
@@ -28,7 +30,7 @@ import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PEAK_BF16_TFLOPS = 989.0  # H100 SXM data sheet, dense bf16 (700 W card): a ceiling, not a measured rate
-RUNS = (("full", None), ("no_loads", "1"), ("no_epilogue", "2"))
+RUNS = (("full", None), ("no_loads", "1"), ("no_epilogue", "2"), ("no_stores", "4"))
 
 
 def gpu_info():
