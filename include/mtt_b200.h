@@ -15,7 +15,8 @@
  *  - "split" tensors: an fp32 value x is carried as two bf16 planes, hi = bf16(x) and
  *    lo = bf16(x - hi), with identical layout. nsplit = 2 uses both planes (3 tensor-core MMAs per
  *    product: hi*hi + hi*lo + lo*hi, ~2^-17 relative error, the parity mode); nsplit = 1 uses only
- *    the hi plane (plain bf16, the speed mode). lo pointers may be NULL when nsplit = 1.
+ *    the hi plane (plain bf16, the speed mode). lo pointers may be NULL when nsplit = 1; an output lo
+ *    plane that is given anyway (mtt_gemm, mtt_attention) is written as bf16(x - hi) in either mode.
  *  - All leading dimensions are in ELEMENTS.
  */
 #ifndef MTT_B200_H_

@@ -257,7 +257,7 @@ attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_const
       uint32_t hv, lv;
       split_pack2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv, hv, lv);
       *reinterpret_cast<uint32_t*>(p.out_hi + off + 8 * i) = hv;
-      if (NSPLIT == 2) *reinterpret_cast<uint32_t*>(p.out_lo + off + 8 * i) = lv;
+      if (NSPLIT == 2 || p.out_lo) *reinterpret_cast<uint32_t*>(p.out_lo + off + 8 * i) = lv;
     }
   }
 }

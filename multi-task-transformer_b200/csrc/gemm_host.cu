@@ -62,7 +62,7 @@ int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensor
   p.out_f32 = d->out_f32;
   p.ldo_f32 = d->ldo_f32;
   p.out_hi = static_cast<__nv_bfloat16*>(d->out_hi);
-  p.out_lo = d->nsplit == 2 ? static_cast<__nv_bfloat16*>(d->out_lo) : nullptr;
+  p.out_lo = static_cast<__nv_bfloat16*>(d->out_lo);  // written whenever given: nsplit = 1 leaves no stale lo plane
   p.ldo_bf = d->ldo_bf;
   p.in_group = d->in_group;
   p.out_group = d->out_group;

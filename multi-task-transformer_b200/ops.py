@@ -181,7 +181,7 @@ def attention(qkv, out, *, B, N, H, scale, prompt_logits=None, T=0):
     nsplit = min(qkv.nsplit, out.nsplit)
     assert qkv.ld == 3 * H * 64 and out.ld == H * 64
     d.qkv_hi, d.qkv_lo = qkv.hi.data_ptr(), (qkv.lo.data_ptr() if nsplit == 2 else 0)
-    d.out_hi, d.out_lo = out.hi.data_ptr(), (out.lo.data_ptr() if nsplit == 2 else 0)
+    d.out_hi, d.out_lo = out.hi.data_ptr(), (out.lo.data_ptr() if out.nsplit == 2 else 0)   # lo written in either mode
     if prompt_logits is not None:
         assert prompt_logits.dtype == torch.float32 and prompt_logits.is_contiguous()
         assert tuple(prompt_logits.shape) == (B, H, T, N)

@@ -104,10 +104,10 @@ def test_gemm_splitk(both, cuda_dev):
         assert relerr(out, want) < 2e-5
 
 
-@pytest.mark.parametrize("variant", [1, 2], ids=["1cta_128x128", "cta_pair_256x256"])
+@pytest.mark.parametrize("variant", [1, 2], ids=["bn128", "bn256"])
 def test_gemm_grouped_equals_separate_launches(both, cuda_dev, variant):
     """mtt_gemm_grouped == the same problems launched one by one on the same kernel variant, bit for bit (linear and
-    3x3 conv, ragged N: the CTA pair narrows its last N tile), and both agree with float64."""
+    3x3 conv, ragged N: the last N tile is partial), and both agree with float64."""
     ops, emu = both
     ops.set_gemm_variant(variant)
     try:
