@@ -17,6 +17,10 @@ heads:
 `TrainStep.step(images, targets)` is the native loop; `TrainStep.apply(images)` is the torch-facing form (one
 autograd.Function: `loss.backward()` runs the reverse pass and hands per-parameter gradients to autograd, so the
 reference loop's criterion, clip_grad_norm_, optimizer and DDP hooks work unchanged).
+`TrainStep.state_dict()` / `load_state_dict()` save and restore the Adam state in torch.optim.Adam's format (the
+checkpoint's 'optimizer' entry, train_utils.py:128, main.py:115-135); the model's own state_dict() is the 'model' entry.
+Every write the kernels make to parameters or BatchNorm statistics bumps their version counters, so eval forwards of the
+model re-pack the trained weights.
 
 Not covered (raise): DEConvHead / Swin / InvPT models, attention or projection dropout (0 in every reference config).
 """
@@ -104,6 +108,10 @@ class TrainStep:
                 self.params.view[n].copy_(p.detach().to(self.dev, torch.float32))
                 p.data = self.params.view[n]
                 p.grad = self.grads.view[n]
+        # the arenas and the BatchNorm statistics are written by kernels torch does not see: their version counters (what
+        # the packed-weight caches and launch plans key on, plans._version) are bumped by hand after every such write
+        self._param_list = [p for _, p in named]
+        self._buffer_list = list(model.buffers())
         self.gnorm = _z((), device=self.dev)
         self.comm = torch.cuda.Stream(device=self.dev) if (self.pg is not None and self.dev.type == "cuda") else None
         self.bucket_elems = int(bucket_mb * (1 << 20) // 4)
@@ -306,7 +314,9 @@ class TrainStep:
         self._level_fwd(3, xfin, logits, rc, acc, B, self.depth - 1)
         oh, ow = self.target if self.target is not None else img.shape[-2:]
         cx["out_hw"] = (oh, ow)
-        return self._heads_fwd(acc, B, oh, ow)
+        out = self._heads_fwd(acc, B, oh, ow)
+        torch.autograd.graph.increment_version(self._buffer_list)        # running statistics (mtt_bn_finalize)
+        return out
 
     def _block_fwd(self, i, X, B, want, scales):
         dev, ns = self.dev, self.ns
@@ -780,6 +790,68 @@ class TrainStep:
             ops.sumsq(self.grads.flat, self.gnorm)
         ops.adam_step(self.params.flat, self.grads.flat, self.m, self.v, step=self.step_no,
                       gnorm_sq=self.gnorm if clip else None, max_norm=self.max_norm or 0.0, grad_scale=gs, **h)
+        torch.autograd.graph.increment_version(self._param_list)
+
+    def _moment(self, flat, name):
+        """Parameter `name`'s slice of a moment arena (self.m / self.v share the parameter arena's layout)."""
+        o, n, shape = self.params.offsets[name]
+        return flat[o:o + n].view(shape)
+
+    def state_dict(self):
+        """The optimizer state as torch.optim.Adam(model.parameters(), ...).state_dict() has it: one param group (the
+        group keys come from a real torch Adam built with self.hyper), parameters indexed in model.parameters() order,
+        state[i] = {'step', 'exp_avg', 'exp_avg_sq'} (copies), no state before the first step. With a process group the
+        moments are the same on every rank."""
+        h = self.hyper
+        sd = torch.optim.Adam(self.model.parameters(), lr=h["lr"], betas=h["betas"], eps=h["eps"],
+                              weight_decay=h["weight_decay"]).state_dict()
+        if self.step_no:
+            sd["state"] = {i: {"step": torch.tensor(float(self.step_no)), "exp_avg": self._moment(self.m, n).clone(),
+                               "exp_avg_sq": self._moment(self.v, n).clone()} for i, n in enumerate(self.names)}
+        return sd
+
+    def load_state_dict(self, sd):
+        """Loads an Adam state dict: what state_dict() returns, what torch.optim.Adam writes for this model (torch 1.10
+        stores 'step' as an int), or that of a fresh optimizer (empty state = step 0). The moments are copied into the
+        arenas in place (a captured step graph stays valid); step count and hyper-parameters come from the group. The
+        parameters themselves are the model's: model.load_state_dict() writes them into the arena."""
+        groups = sd["param_groups"]
+        if len(groups) != 1:
+            raise ValueError(f"TrainStep.load_state_dict: {len(groups)} param groups; TrainStep keeps one")
+        g = groups[0]
+        for k in ("amsgrad", "maximize", "decoupled_weight_decay"):
+            if g.get(k, False):
+                raise ValueError(f"TrainStep.load_state_dict: '{k}' is set; TrainStep runs plain Adam")
+        ids = list(g["params"])
+        if len(ids) != len(self.names):
+            raise ValueError(f"TrainStep.load_state_dict: {len(ids)} parameters in the group, the model has "
+                             f"{len(self.names)}")
+        state = sd["state"]
+        have = [i for i in ids if i in state]
+        if have and len(have) != len(ids):
+            raise ValueError(f"TrainStep.load_state_dict: state for {len(have)} of {len(ids)} parameters (TrainStep keeps "
+                             "state for all or none)")
+        steps = sorted({int(float(state[i]["step"])) for i in have})
+        if len(steps) > 1:
+            raise ValueError(f"TrainStep.load_state_dict: step counts {steps} differ between parameters (TrainStep "
+                             "keeps one)")
+        for i, n in zip(ids, self.names):
+            shape = self.params.offsets[n][2]
+            for k in ("exp_avg", "exp_avg_sq"):
+                if have and tuple(state[i][k].shape) != shape:
+                    raise ValueError(f"TrainStep.load_state_dict: {k} of parameter {i} ({n}) has shape "
+                                     f"{tuple(state[i][k].shape)}, the parameter {shape}")
+        with torch.no_grad():
+            if have:
+                for i, n in zip(ids, self.names):
+                    self._moment(self.m, n).copy_(state[i]["exp_avg"])
+                    self._moment(self.v, n).copy_(state[i]["exp_avg_sq"])
+            else:
+                self.m.zero_()
+                self.v.zero_()
+        self.step_no = steps[0] if steps else 0
+        self.hyper = dict(lr=float(g["lr"]), betas=tuple(float(b) for b in g["betas"]), eps=float(g["eps"]),
+                          weight_decay=float(g["weight_decay"]))
 
     def step(self, images, targets, criterion, tasks=None):
         """One iteration of train_utils.py:34-51 with `criterion` = mtt_b200.losses.MultiTaskLoss (device kernels):
@@ -827,6 +899,7 @@ class TrainStep:
         for t, v in targets.items():
             gy[t].copy_(v, non_blocking=True)
         g.replay()
+        torch.autograd.graph.increment_version(self._buffer_list)        # the replayed forward's running statistics
         return loss
 
     def apply(self, images):
