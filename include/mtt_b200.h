@@ -426,6 +426,46 @@ int mtt_loss_l1_grad(const float* pred, const float* label, int32_t B, int32_t C
                      float ignore_index, int32_t use_ignore, int32_t normalize, const float* grad_scale, float* dpred,
                      const void* workspace, mtt_stream_t stream);
 
+/* ---- evaluation meters (the reference's PerformanceMeter, TP/evaluation/evaluate_utils.py:13-66) ------------------
+ * Each *_update enqueues ONE kernel that adds a batch's statistics into `state`, a caller-owned device buffer of
+ * mtt_meter_state_bytes(kind, n) bytes (8-byte aligned; n = classes for CONFUSION, thresholds for SALIENCY, ignored
+ * otherwise); mtt_meter_reset zeroes it with a cudaMemsetAsync on `stream`. Nothing is allocated or synchronised, so
+ * updates can be captured in a CUDA graph; the score formulas run on the host over one copy of the state (layouts in
+ * csrc/metrics.cu). Integer counters are int64; float sums are fp64, reduced in a fixed order (bitwise reproducible).
+ * Inputs are predict()'s outputs (= the reference's get_output, TP/utils/utils.py:27-63) and the labels as the
+ * reference's loader yields them: fp32 [B,C,H,W], ignore_index marking ignored pixels.
+ *   CONFUSION  pred int64 [B,H,W] class map, label [B,1,H,W]; SemsegMeter eval_semseg.py:70-81 and HumanPartsMeter
+ *              eval_human_parts.py:33-42 (n_classes <= 64).
+ *   SALIENCY   pred fp32 [B,H,W] (255 * probability), label [B,1,H,W]; SaliencyMeter eval_sal.py:21-60:
+ *              prob = sigmoid(pred / 255), counts per threshold (device array of n_thresholds <= 32 floats).
+ *   NORMALS    pred fp32 [B,H,W,3] ((n + 1) * 255 / 2), label [B,3,H,W]; NormalsMeter eval_normals.py:33-45.
+ *   DEPTH      pred fp32 with B*H*W elements, label [B,1,H,W]; valid = min_depth < gt < max_depth when use_range
+ *              (TP eval_depth.py:36), gt != ignore_index otherwise (IP eval_depth.py DepthMeter). Values <= 0 count as
+ *              1e-9 (:41-42); unlike the reference, the inputs are not modified.
+ *   EDGE       pred fp32 [B,H,W] (255 * sigmoid), label [B,1,H,W]; EdgeMeter eval_edge.py:21-31 with a fixed
+ *              pos_weight in [0, 1). */
+enum mtt_meter_kind {
+  MTT_METER_CONFUSION = 0,
+  MTT_METER_SALIENCY = 1,
+  MTT_METER_NORMALS = 2,
+  MTT_METER_DEPTH = 3,
+  MTT_METER_EDGE = 4
+};
+/* 0 (with the error text set) for an unknown kind or a size over the capacity */
+size_t mtt_meter_state_bytes(int32_t kind, int32_t n);
+int mtt_meter_reset(void* state, int32_t kind, int32_t n, mtt_stream_t stream);
+int mtt_meter_confusion_update(const int64_t* pred, const float* label, int32_t B, int32_t H, int32_t W,
+                               int32_t n_classes, float ignore_index, void* state, mtt_stream_t stream);
+int mtt_meter_saliency_update(const float* pred, const float* label, int32_t B, int32_t H, int32_t W,
+                              const float* thresholds, int32_t n_thresholds, float ignore_index, void* state,
+                              mtt_stream_t stream);
+int mtt_meter_normals_update(const float* pred_nhwc, const float* label, int32_t B, int32_t H, int32_t W,
+                             float ignore_index, void* state, mtt_stream_t stream);
+int mtt_meter_depth_update(const float* pred, const float* label, int32_t B, int32_t H, int32_t W, int32_t use_range,
+                           float min_depth, float max_depth, float ignore_index, void* state, mtt_stream_t stream);
+int mtt_meter_edge_update(const float* pred, const float* label, int32_t B, int32_t H, int32_t W, float pos_weight,
+                          float ignore_index, void* state, mtt_stream_t stream);
+
 /* ---- BEV IoU of rotated boxes and NMS (SURVEY.md 8f N4) ---------------------------------------------------------
  * Replaces the reference's native extension TP/detection_toolbox/iou3d (iou3d_kernel.cu:253-439, iou3d.cpp:51-202).
  * Boxes are [x1, y1, x2, y2, ry] fp32 rows on the device. mtt_boxes_bev_pairwise: out[a, b] = overlap area (mode 0,

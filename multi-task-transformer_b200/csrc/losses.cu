@@ -12,6 +12,7 @@
 #include <math.h>
 
 #include "host_common.h"
+#include "loss_terms.cuh"
 
 namespace mtt {
 
@@ -145,8 +146,8 @@ ce_kernel(const float* __restrict__ pred, const float* __restrict__ label, long 
 }
 
 // ---- balanced binary cross entropy ------------------------------------------------------------------------------------
-// per = w y softplus(-x) + (1 - w)(1 - y) softplus(x), mean over kept entries; w = pos_weight, or (hed) n_neg / n_valid.
-__device__ __forceinline__ float softplusf(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
+// per = w y softplus(-x) + (1 - w)(1 - y) softplus(x) (balanced_bce_term), mean over kept entries; w = pos_weight, or
+// (hed) n_neg / n_valid.
 
 template <bool GRAD>
 __global__ void __launch_bounds__(kLossThreads)
@@ -163,7 +164,7 @@ bce_kernel(const float* __restrict__ pred, const float* __restrict__ label, long
     const float y = label[i], x = pred[i];
     const bool keep = y != ignore;
     if (!GRAD) {
-      if (keep) acc += (double)(w * y * softplusf(-x) + (1.f - w) * (1.f - y) * softplusf(x));
+      if (keep) acc += (double)balanced_bce_term(x, y, w);
     } else {
       const float s = 1.f / (1.f + expf(-x));
       dpred[i] = keep ? (-(w * y) * (1.f - s) + (1.f - w) * (1.f - y) * s) * gs : 0.f;

@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmtt_sm90.so")
 
 ACT_NONE, ACT_GELU, ACT_RELU = 0, 1, 2
+METER_CONFUSION, METER_SALIENCY, METER_NORMALS, METER_DEPTH, METER_EDGE = 0, 1, 2, 3, 4
 
 
 class GemmDesc(C.Structure):
@@ -131,6 +132,14 @@ SYMBOLS = {
     "mtt_loss_balanced_bce_grad": (C.c_int, [_vp, _vp, _i64, _f32, _f32, _i32, _vp, _vp, _vp, _vp]),
     "mtt_loss_l1": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _i32, _i32, _vp, _vp, _vp]),
     "mtt_loss_l1_grad": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    # evaluation meters (csrc/metrics.cu)
+    "mtt_meter_state_bytes": (C.c_size_t, [_i32, _i32]),
+    "mtt_meter_reset": (C.c_int, [_vp, _i32, _i32, _vp]),
+    "mtt_meter_confusion_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "mtt_meter_saliency_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _i32, _f32, _vp, _vp]),
+    "mtt_meter_normals_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "mtt_meter_depth_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _f32, _vp, _vp]),
+    "mtt_meter_edge_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _f32, _f32, _vp, _vp]),
     "mtt_boxes_bev_pairwise": (C.c_int, [_vp, _i32, _vp, _i32, _i32, _vp, _vp]),
     "mtt_nms_workspace_bytes": (C.c_size_t, [_i32]),
     "mtt_nms_bev": (C.c_int, [_vp, _i32, _f32, _i32, _vp, _vp, _vp, C.c_size_t, _vp]),

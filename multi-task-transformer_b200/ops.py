@@ -308,6 +308,85 @@ def bilinear_postproc(x, ld_in, B, h, w, Cdim, H2, W2, kind, out):
     _L.check(rc, "mtt_bilinear_postproc")
 
 
+METER_CONFUSION, METER_SALIENCY, METER_NORMALS, METER_DEPTH, METER_EDGE = (
+    _L.METER_CONFUSION, _L.METER_SALIENCY, _L.METER_NORMALS, _L.METER_DEPTH, _L.METER_EDGE)
+
+
+def meter_state_bytes(kind, n=0):
+    """Bytes of device state a meter of `kind` needs (n = classes or thresholds); ValueError when the library refuses
+    the kind or the size."""
+    nb = int(_L.load().mtt_meter_state_bytes(int(kind), int(n)))
+    if nb == 0:
+        raise ValueError(_L.load().mtt_last_error().decode("utf-8", "replace"))
+    return nb
+
+
+def meter_reset(state, kind, n=0):
+    _L.check(_L.load().mtt_meter_reset(_ptr(state), int(kind), int(n), _stream()), "mtt_meter_reset")
+
+
+def _meter_inputs(what, pred, pred_dtype, pred_shape, label, label_channels, state):
+    """Validates a meter update's tensors before any launch: dtypes, shapes (pred_shape(B, H, W) from the label's
+    [B, label_channels, H, W]), contiguity and device. Returns (B, H, W)."""
+    if label.dtype != torch.float32 or label.dim() != 4 or label.shape[1] != label_channels:
+        raise ValueError(f"{what}: label must be fp32 [B,{label_channels},H,W], got {label.dtype} {tuple(label.shape)}")
+    B, _, H, W = (int(s) for s in label.shape)
+    if pred.dtype != pred_dtype or tuple(pred.shape) != pred_shape(B, H, W):
+        raise ValueError(f"{what}: prediction must be {pred_dtype} {pred_shape(B, H, W)} for a label of shape "
+                         f"{tuple(label.shape)}, got {pred.dtype} {tuple(pred.shape)}")
+    if not (pred.is_cuda and label.is_cuda and state.is_cuda):
+        raise RuntimeError(f"{what}: the meters run on the GPU only; got tensors on {pred.device} / {label.device}")
+    if not (pred.is_contiguous() and label.is_contiguous()):
+        raise ValueError(f"{what}: prediction and label must be contiguous")
+    return B, H, W
+
+
+def meter_confusion_update(pred, label, n_classes, ignore_index, state):
+    """pred int64 [B,H,W] class map, label fp32 [B,1,H,W]."""
+    B, H, W = _meter_inputs("meter_confusion_update", pred, torch.int64, lambda b, h, w: (b, h, w), label, 1, state)
+    rc = _L.load().mtt_meter_confusion_update(_ptr(pred), _ptr(label), B, H, W, int(n_classes), float(ignore_index),
+                                              _ptr(state), _stream())
+    _L.check(rc, "mtt_meter_confusion_update")
+
+
+def meter_saliency_update(pred, label, thresholds, ignore_index, state):
+    """pred fp32 [B,H,W] (255 * probability), label fp32 [B,1,H,W], thresholds fp32 on the device."""
+    B, H, W = _meter_inputs("meter_saliency_update", pred, torch.float32, lambda b, h, w: (b, h, w), label, 1, state)
+    assert thresholds.is_cuda and thresholds.dtype == torch.float32 and thresholds.is_contiguous()
+    rc = _L.load().mtt_meter_saliency_update(_ptr(pred), _ptr(label), B, H, W, _ptr(thresholds), thresholds.numel(),
+                                             float(ignore_index), _ptr(state), _stream())
+    _L.check(rc, "mtt_meter_saliency_update")
+
+
+def meter_normals_update(pred, label, ignore_index, state):
+    """pred fp32 [B,H,W,3] (predict()'s normals), label fp32 [B,3,H,W]."""
+    B, H, W = _meter_inputs("meter_normals_update", pred, torch.float32, lambda b, h, w: (b, h, w, 3), label, 3, state)
+    rc = _L.load().mtt_meter_normals_update(_ptr(pred), _ptr(label), B, H, W, float(ignore_index), _ptr(state),
+                                            _stream())
+    _L.check(rc, "mtt_meter_normals_update")
+
+
+def meter_depth_update(pred, label, state, *, min_depth=None, max_depth=None, ignore_index=255):
+    """pred fp32 [B,H,W,1] (predict()'s depth) or [B,H,W], label fp32 [B,1,H,W]. The mask is min_depth < gt <
+    max_depth when both bounds are given, gt != ignore_index otherwise."""
+    shape = (lambda b, h, w: (b, h, w, 1)) if pred.dim() == 4 else (lambda b, h, w: (b, h, w))
+    B, H, W = _meter_inputs("meter_depth_update", pred, torch.float32, shape, label, 1, state)
+    use_range = min_depth is not None and max_depth is not None
+    rc = _L.load().mtt_meter_depth_update(_ptr(pred), _ptr(label), B, H, W, int(use_range),
+                                          float(min_depth) if use_range else 0.0,
+                                          float(max_depth) if use_range else 0.0, float(ignore_index), _ptr(state),
+                                          _stream())
+    _L.check(rc, "mtt_meter_depth_update")
+
+
+def meter_edge_update(pred, label, pos_weight, ignore_index, state):
+    """pred fp32 [B,H,W] (255 * sigmoid), label fp32 [B,1,H,W]."""
+    B, H, W = _meter_inputs("meter_edge_update", pred, torch.float32, lambda b, h, w: (b, h, w), label, 1, state)
+    rc = _L.load().mtt_meter_edge_update(_ptr(pred), _ptr(label), B, H, W, float(pos_weight), float(ignore_index),
+                                         _ptr(state), _stream())
+    _L.check(rc, "mtt_meter_edge_update")
+
+
 IMAGENET_MEAN = (0.485, 0.456, 0.406)   # TP/inference.py:99,107
 IMAGENET_STD = (0.229, 0.224, 0.225)
 
