@@ -39,6 +39,18 @@ class Split:
         alloc = torch.zeros if zero else torch.empty
         self.buf = alloc((self.nsplit, self.rows, self.ld), dtype=torch.bfloat16, device=device)
 
+    @classmethod
+    def from_planes(cls, buf, cols):
+        """The Split over an existing [nsplit, rows, ld] bf16 tensor (shares its storage)."""
+        sp = cls.__new__(cls)
+        sp.buf, sp.cols = buf, int(cols)
+        sp.nsplit, sp.rows, sp.ld = buf.shape
+        return sp
+
+    def rows_view(self, r0, n):
+        """Rows [r0, r0 + n) as a Split (shares storage)."""
+        return Split.from_planes(self.buf[:, r0:r0 + n], self.cols)
+
     @property
     def hi(self):
         return self.buf[0]
@@ -83,19 +95,17 @@ def layernorm(x, gamma, beta, eps, out_f32=None, out_split=None):
     _L.check(rc, "mtt_layernorm")
 
 
-def gemm(a, w, *, M=None, N=None, K=None, bias=None, act=ACT_NONE, residual=None, res_row_mod=0,
-         out_f32=None, out_split=None, out_col_offset=0, regroup=None, conv=None, a_row_offset=0,
-         a_gather=None, w_col_offset=0, a_col_offset=0, w_row_offset=0, out_row_offset=0, sk_ws=None):
+def gemm(a, w, *, sk_ws=None, **kw):
     """D = act(A @ W^T + bias) + residual on the wgmma GEMM.
 
     a: Split [M, K] (or NHWC activation [B*H*W, C] when ``conv=(B, H, W, ksize, dil)``);
     w: Split [N, K] (conv: [N, ksize*ksize*cin_pad]); outputs: fp32 tensor and/or Split.
     regroup=(in_group, out_group, out_offset[, row_stride]) scatters output rows; a_gather=(group_rows,
     group_stride) gathers A rows in groups (M must be given); w_col_offset selects a K-slice of a wider packed W.
-    sk_ws: optional stream-K workspace (streamk_workspace(device)); see mtt_gemm_desc.sk_ws."""
+    sk_ws: optional stream-K workspace (streamk_workspace(device)); see mtt_gemm_desc.sk_ws.
+    The keyword arguments and their defaults are _fill_gemm_desc's."""
     d = _L.GemmDesc()
-    _fill_gemm_desc(d, a, w, M, N, K, bias, act, residual, res_row_mod, out_f32, out_split, out_col_offset, regroup, conv,
-                    a_row_offset, a_gather, w_col_offset, a_col_offset, w_row_offset, out_row_offset)
+    _fill_gemm_desc(d, a, w, **kw)
     if sk_ws is not None:
         d.sk_ws, d.sk_ws_bytes = sk_ws.data_ptr(), sk_ws.numel()
     rc = _L.load().mtt_gemm(C.byref(d), _stream())
@@ -107,11 +117,7 @@ def gemm_grouped(calls):
     tensors -- as ONE persistent launch (mtt_gemm_grouped)."""
     arr = (_L.GemmDesc * len(calls))()
     for d, (a, w, kw) in zip(arr, calls):
-        k = dict(M=None, N=None, K=None, bias=None, act=ACT_NONE, residual=None, res_row_mod=0, out_f32=None,
-                 out_split=None, out_col_offset=0, regroup=None, conv=None, a_row_offset=0, a_gather=None, w_col_offset=0,
-                 a_col_offset=0, w_row_offset=0, out_row_offset=0)
-        k.update(kw)
-        _fill_gemm_desc(d, a, w, **k)
+        _fill_gemm_desc(d, a, w, **kw)
     rc = _L.load().mtt_gemm_grouped(arr, len(calls), _stream())
     _L.check(rc, "mtt_gemm_grouped")
 
@@ -133,8 +139,9 @@ def gemm_splitk(a, w, partial, out_f32, *, K, bias=None, chunks):
     _L.check(rc, "mtt_sum_partials")
 
 
-def _fill_gemm_desc(d, a, w, M, N, K, bias, act, residual, res_row_mod, out_f32, out_split, out_col_offset, regroup, conv,
-                    a_row_offset, a_gather, w_col_offset, a_col_offset=0, w_row_offset=0, out_row_offset=0):
+def _fill_gemm_desc(d, a, w, *, M=None, N=None, K=None, bias=None, act=ACT_NONE, residual=None, res_row_mod=0,
+                    out_f32=None, out_split=None, out_col_offset=0, regroup=None, conv=None, a_row_offset=0,
+                    a_gather=None, w_col_offset=0, a_col_offset=0, w_row_offset=0, out_row_offset=0):
     """w_row_offset / out_row_offset: first row of the B operand / of the split output (pointer offsets): lets one
     buffer hold the operands of several (batch, head) problems of a grouped launch."""
     nsplit = min(a.nsplit, w.nsplit)
@@ -508,10 +515,7 @@ def ws_split_view(ws, byte_offset, rows, cols, nsplit):
     """The Split living at `byte_offset` of a workspace, laid out as block_ops.cu does: [nsplit][rows][pad8(cols)]."""
     ld = round_up(cols, 8)
     n = nsplit * rows * ld
-    sp = Split.__new__(Split)
-    sp.rows, sp.cols, sp.ld, sp.nsplit = rows, cols, ld, nsplit
-    sp.buf = ws[byte_offset: byte_offset + 2 * n].view(torch.bfloat16).view(nsplit, rows, ld)
-    return sp
+    return Split.from_planes(ws[byte_offset: byte_offset + 2 * n].view(torch.bfloat16).view(nsplit, rows, ld), cols)
 
 
 def ln_qkv(x, gamma, beta, eps, wqkv, bias, qkv, ws):

@@ -113,18 +113,23 @@ def _launch_block(sp, w, want_logits):
     ops.ln_mlp_residual(sp.xs, w.n2w, w.n2b, w.eps, w.fc1, w.fc1_b, w.fc2, w.fc2_b, sp.ws_mlp)  # :274, :277
 
 
+def prompt_row_chunks(B, T):
+    """(b0, nb): images [b0, b0 + nb) per GEMM launch over prompt rows: their T prompt rows each form one gathered
+    128-row A tile."""
+    bstep = max(1, 128 // T)
+    for b0 in range(0, B, bstep):
+        yield b0, min(bstep, B - b0)
+
+
 def _launch_chan_path(sp, w, want_logits):
     B, N, T, C = sp.B, sp.N, sp.T, sp.C
-    bstep = max(1, 128 // T)      # images per launch: their T prompt rows form one gathered 128-row A tile
-    for b0 in range(0, B, bstep):
-        nb = min(bstep, B - b0)
+    for b0, nb in prompt_row_chunks(B, T):
         ops.gemm(sp.xn, w.tt, M=nb * T, bias=w.tt_b, a_gather=(T, N), a_row_offset=b0 * N,
                  out_f32=sp.cp, out_split=sp.cps, regroup=(nb * T, nb * T, b0 * T))           # :219 token_trans
     if want_logits:
         ops.chan_logits(sp.cp, sp.xn, sp.rc, B=B, N=N, T=T, Cdim=C, gh=sp.gh, gw=sp.gw,
                         nh=sp.nh, nw=sp.nw)                                                   # :236-246
-    for b0 in range(0, B, bstep):
-        nb = min(bstep, B - b0)
+    for b0, nb in prompt_row_chunks(B, T):
         ops.gemm(sp.cps, w.tt1, M=nb * T, bias=w.tt1_b, a_row_offset=b0 * T, residual=sp.xs,
                  out_f32=sp.xs, regroup=(T, N, b0 * N))                                       # :250 token_trans1
 

@@ -30,6 +30,7 @@ import torch
 
 from . import ops
 from .ops import ACT_GELU, ACT_NONE, Split, round_up
+from .taskprompter import ConvHead, TaskPrompter, TaskPrompterWrapper, prompt_row_chunks
 
 __all__ = ["TrainStep"]
 
@@ -63,7 +64,6 @@ class TrainStep:
 
     def __init__(self, model, *, lr=2e-5, betas=(0.9, 0.999), eps=1e-8, weight_decay=1e-6, max_norm=10.0, nsplit=2,
                  process_group=None, bucket_mb=64, use_graph=False):
-        from .taskprompter import ConvHead, TaskPrompter, TaskPrompterWrapper
         if not isinstance(model, TaskPrompterWrapper) or not isinstance(model.backbone, TaskPrompter):
             raise NotImplementedError("mtt_b200 TrainStep: only the ViT TaskPrompter is covered (SURVEY.md 8f N1)")
         for t in model.tasks:
@@ -115,7 +115,7 @@ class TrainStep:
         self.gnorm = _z((), device=self.dev)
         self.comm = torch.cuda.Stream(device=self.dev) if (self.pg is not None and self.dev.type == "cuda") else None
         self.bucket_elems = int(bucket_mb * (1 << 20) // 4)
-        self._pending = []
+        self._pending, self._done = [], set()
         self.ctx = None
         # use_graph: step() captures forward + criterion + reverse pass (about 5000 launches) into ONE CUDA graph per input
         # shape and replays it; clip + Adam stay outside (their bias-correction scalars change every step)
@@ -184,59 +184,67 @@ class TrainStep:
         self._gemm(a, w, M=M, N=N, K=K, bias=bias, out_f32=out, **kw)
         return out
 
-    def _lin_bwd(self, dy, a_s, name, *, M, N, K, need_dx=True, dx_residual=None, dx_out=None, wkey=None, gW=None,
-                 bias_name="auto", dy_s=None):
-        """Y [M,N] = A [M,K] W^T + b. dy fp32 [M,N]; a_s Split [M,K]. Accumulates dW, db; returns dA (fp32 [M,K])."""
-        wkey = name if wkey is None else wkey
-        gW = self.G_(name).reshape(N, -1) if gW is None else gW
-        dyT = Split(N, M, self.dev, self.ns)
-        ops.transpose_split(dy, dyT, B=1, L=M, Cdim=N)
-        aT = ops.transpose_planes(a_s, R=M, Ccols=K)
-        self._gemm(dyT, aT, M=N, N=K, K=M, residual=gW, out_f32=gW)                       # dW += dY^T A
-        if bias_name == "auto":
-            bias_name = name[:-len("weight")] + "bias"
-        if bias_name is not None:
-            ops.colsum(dy, self.G_(bias_name), accumulate=True, rows=M)
-        if not need_dx:
-            return None
+    def _gemms(self, calls):
+        """[(a, w, kwargs)]: one problem goes through self._gemm (it has the step's stream-K workspace, which a grouped
+        launch cannot take), several go out as grouped launches."""
+        if len(calls) == 1:
+            a, w, kw = calls[0]
+            self._gemm(a, w, **kw)
+        else:
+            _grouped(calls)
+
+    def _wb(self, layer):
+        """The _lin_bwd item of the Linear / 1x1 Conv2d `layer`: (dW as [N, K], db, key of its weight in self.WT)."""
+        gW = self.G_(layer + ".weight")
+        return gW.reshape(gW.shape[0], -1), self.G_(layer + ".bias"), layer + ".weight"
+
+    def _lin_bwd(self, dy, a_s, items, *, M, N, K, dyT=None, aT=None, dy_s=None, dy_rows=None, dx=None,
+                 accumulate_dx=False):
+        """The adjoint of len(items) problems Y_t = A_t W_t^T + b_t stacked by rows: dy fp32 [T*M, N] (any row stride),
+        a_s Split [T*M, K]; items[t] = (dW view [N, K], db view or None, key of W_t in self.WT or None).
+        dW_t += dY_t^T A_t and db_t += colsum(dY_t) accumulate. With a key, dA_t = dY_t W_t goes to rows t*M.. of dx (fp32
+        [T*M, K]; None: a new tensor; accumulate_dx: added to what dx holds). Returns (dA or None, dyT, dy_s): the
+        transposed / split dY can serve a second call on the same dY.
+        A caller whose operands are gathered from a wider buffer passes them in: dyT Split [T*N, M]; aT Split [T*K, M], or
+        [K, T*M] with the T blocks side by side (im2col3x3_t of a stacked input); dy_s Split [T*M, N]; and dy_rows =
+        (in_group, src_group, src_offset), the rows of dY inside dy as ops.split_rows maps them."""
+        Tn, dev, ns = len(items), self.dev, self.ns
+        if dyT is None:
+            dyT = Split(Tn * N, M, dev, ns)
+            ops.transpose_split(dy, dyT, B=Tn, L=M, Cdim=N)
+        if aT is None:
+            aT = ops.transpose_planes(a_s, B=Tn, R=M, Ccols=K)
+        stacked = aT.rows == Tn * K
+        self._gemms([(dyT, aT, dict(M=N, N=K, K=M, a_row_offset=t * N, w_row_offset=t * K if stacked else 0,
+                                    w_col_offset=0 if stacked else t * M, residual=gW, out_f32=gW))
+                     for t, (gW, _, _) in enumerate(items)])                                      # dW += dY^T A
+        for t, (_, gb, _) in enumerate(items):
+            if gb is not None:
+                in_group, src_group, src_offset = dy_rows or ((M, M, t * M) if Tn > 1 else (0, 0, 0))
+                ops.colsum(dy, gb, accumulate=True, rows=M, in_group=in_group, src_group=src_group, src_offset=src_offset)
+        if items[0][2] is None:
+            return None, dyT, dy_s
         dy_s = self._S(dy) if dy_s is None else dy_s
-        if dx_out is None:
-            dx_out = _e(M, K, device=self.dev)
-        self._gemm(dy_s, self.WT[wkey], M=M, N=K, K=N, residual=dx_residual, out_f32=dx_out)  # dA = dY W
-        return dx_out
+        if dx is None:
+            dx = _e(Tn * M, K, device=dev)
+        self._gemms([(dy_s, self.WT[key], dict(M=M, N=K, K=N, a_row_offset=t * M, out_f32=dx[t * M:(t + 1) * M],
+                                               residual=dx[t * M:(t + 1) * M] if accumulate_dx else None))
+                     for t, (_, _, key) in enumerate(items)])                                     # dA = dY W
+        return dx, dyT, dy_s
 
     # ---- forward -------------------------------------------------------------------------------------------------------
-    def _drop_scales(self, B, rand=None):
-        """Per block the two row-scale vectors [B*N] of the joint stream (attention / MLP residual), or None. `rand`:
-        optional iterator of the uniform [B,1,1] draws to use instead of torch.rand (tests replay the reference's)."""
-        if rand is None:
-            return self._drop_scales_batched(B)
-        out = []
-        for i in range(self.depth):
-            dp = self.drop_path[i]
-            if dp == 0.0:
-                out.append((None, None))
-                continue
-            keep = 1.0 - dp
-            draw = lambda: next(rand).to(self.dev, torch.float32)
-            # reference call order (taskprompter.py:273,274,276,277): x attn, x mlp, prompts attn, prompts mlp
-            r = [torch.floor(keep + draw()) / keep for _ in range(4)]
-            sa = torch.empty(B, self.N, dtype=torch.float32, device=self.dev)
-            sm = torch.empty_like(sa)
-            sa[:, self.T:], sa[:, :self.T] = r[0].view(B, 1), r[2].view(B, 1)
-            sm[:, self.T:], sm[:, :self.T] = r[1].view(B, 1), r[3].view(B, 1)
-            out.append((sa.view(-1), sm.view(-1)))
-        return out
-
-    def _drop_scales_batched(self, B):
-        """The same per-sample masks (timm DropPath: floor(keep + U[0,1)) / keep per sample and residual branch) for ALL
-        blocks from one torch.rand call: ~8 launches per step instead of ~20 per block (1.2 ms of launch time at depth 24)."""
+    def _drop_scales_batched(self, B, u=None):
+        """Per block the two row-scale vectors [B*N] of the joint stream (attention / MLP residual), or (None, None) where
+        the rate is 0: timm DropPath's per-sample masks (floor(keep + U[0,1)) / keep per sample and residual branch) for ALL
+        blocks from one torch.rand call, ~8 launches per step instead of ~20 per block (1.2 ms of launch time at depth 24).
+        `u`: the uniforms [blocks with a non-zero rate, 4, B] to use instead of torch.rand."""
         act = [i for i in range(self.depth) if self.drop_path[i] > 0.0]
         out = [(None, None)] * self.depth
         if not act:
             return out
         keep = self._dp_keep        # device tensor made at construction: nothing here may copy from the host (graph capture)
-        u = torch.rand((len(act), 4, B), dtype=torch.float32, device=self.dev)   # (block, [x attn, x mlp, prompts attn, prompts mlp], sample)
+        if u is None:      # (block, [x attn, x mlp, prompts attn, prompts mlp], sample)
+            u = torch.rand((len(act), 4, B), dtype=torch.float32, device=self.dev)
         r = torch.floor(keep + u) / keep
         s = torch.empty(len(act), 2, B, self.N, dtype=torch.float32, device=self.dev)    # (block, [attn, mlp], sample, token)
         s[:, :, :, self.T:] = r[:, 0:2, :, None]
@@ -278,7 +286,10 @@ class TrainStep:
         return dx
 
     def forward(self, img, drop_rand=None):
-        """images fp32 [B,3,H,W] -> {task: fp32 [B,n_out,H,W]} in train mode; keeps what the reverse pass needs."""
+        """images fp32 [B,3,H,W] -> {task: fp32 [B,n_out,H,W]} in train mode; keeps what the reverse pass needs.
+        `drop_rand`: optional list of the uniform [B,1,1] DropPath draws to use instead of torch.rand, in the reference's
+        call order (taskprompter.py:273,274,276,277: x attn, x mlp, prompts attn, prompts mlp per block with a non-zero
+        rate); tests replay the reference's."""
         dev, ns = self.dev, self.ns
         B = img.shape[0]
         T, P, N, C, H = self.T, self.P, self.N, self.C, self.H
@@ -296,7 +307,11 @@ class TrainStep:
         self._gemm(cols, W[bbp + "patch_embed.proj.weight"], bias=self.P_(bbp + "patch_embed.proj.bias"), residual=pos,
                  res_row_mod=P, out_f32=X, regroup=(P, N, T))
         ops.broadcast_rows(self.P_(bbp + "task_prompts"), X, B, N)
-        scales = self._drop_scales(B, iter(drop_rand) if drop_rand is not None else None)
+        n_act = sum(d > 0.0 for d in self.drop_path)
+        u = None
+        if drop_rand is not None and n_act:
+            u = torch.stack([r.reshape(B) for r in drop_rand[:4 * n_act]]).to(dev, torch.float32).view(n_act, 4, B)
+        scales = self._drop_scales_batched(B, u)
         acc = _z(T, B * P, self.f_ld, device=dev)
         logits = rc = None
         for i in range(self.depth):
@@ -336,17 +351,14 @@ class TrainStep:
         # channel-prompt path on the prompt rows (taskprompter.py:217-250)
         cp = _e(B * T, P, device=dev)
         cps = Split(B * T, P, dev, ns)
-        bstep = max(1, 128 // T)
-        for b0 in range(0, B, bstep):
-            nb = min(bstep, B - b0)
+        for b0, nb in prompt_row_chunks(B, T):
             self._gemm(xn, W[b + "attn.token_trans.weight"], M=nb * T, bias=self.P_(b + "attn.token_trans.bias"),
                      a_gather=(T, N), a_row_offset=b0 * N, out_f32=cp, out_split=cps, regroup=(nb * T, nb * T, b0 * T))
         rc = None
         if want:
             rc = _e(B, T, C, self.nh, self.nw, device=dev)
             ops.chan_logits(cp, xn, rc, B=B, N=N, T=T, Cdim=C, gh=self.gh, gw=self.gw, nh=self.nh, nw=self.nw)
-        for b0 in range(0, B, bstep):
-            nb = min(bstep, B - b0)
+        for b0, nb in prompt_row_chunks(B, T):
             self._gemm(cps, W[b + "attn.token_trans1.weight"], M=nb * T, bias=self.P_(b + "attn.token_trans1.bias"),
                      a_row_offset=b0 * T, residual=o, out_f32=o, regroup=(T, N, b0 * N))
         X1 = _e(M, C, device=dev)
@@ -377,7 +389,7 @@ class TrainStep:
         rows = lambda t: dict(a_row_offset=t * Mp)
         ys, yc = Split(T * Mp, C, dev, ns), Split(T * Mp, C, dev, ns)
         for t in range(T):
-            ops.gate_split(Xsrc, N, T, logits, rc, t, _rows_view(ys, t * Mp, Mp), _rows_view(yc, t * Mp, Mp), B=B, T=T, N=N,
+            ops.gate_split(Xsrc, N, T, logits, rc, t, ys.rows_view(t * Mp, Mp), yc.rows_view(t * Mp, Mp), B=B, T=T, N=N,
                            H=H, Cdim=C, gh=self.gh, gw=self.gw, nh=self.nh, nw=self.nw)
         s_s, c_s = Split(T * Mp, e, dev, ns), Split(T * Mp, e, dev, ns)
         _grouped([(ys, W[ps[t] + "weight"], dict(M=Mp, bias=self.P_(ps[t] + "bias"), out_split=s_s, out_row_offset=t * Mp,
@@ -394,7 +406,7 @@ class TrainStep:
         _grouped([(y0s, W[pf[t] + "1.weight"], dict(M=Mp, N=f, K=f, bias=self.P_(pf[t] + "1.bias"), out_f32=y1[t],
                                                     conv=(B, self.gh, self.gw, 3, 1), **rows(t))) for t in range(T)])
         y2s = Split(T * Mp, f, dev, ns)
-        bn = [self._bn_fwd(y1[t], pf[t] + "2", ACT_GELU, _rows_view(y2s, t * Mp, Mp)) for t in range(T)]
+        bn = [self._bn_fwd(y1[t], pf[t] + "2", ACT_GELU, y2s.rows_view(t * Mp, Mp)) for t in range(T)]
         F_ = _z(T, Mp, self.f_ld, device=dev)
         _grouped([(y2s, W[pf[t] + "4.weight"], dict(M=Mp, bias=self.P_(pf[t] + "4.bias"), out_f32=F_[t][:, :f], **rows(t)))
                   for t in range(T)])
@@ -425,13 +437,13 @@ class TrainStep:
         up = _e(T, M4, f, device=dev)
         ups = Split(T * M4, f, dev, ns)
         for t in range(T):
-            ops.bilinear(acc[t], self.f_ld, B, self.gh, self.gw, f, h4, w4, out_f32=up[t], out_split=_rows_view(ups, t * M4, M4))
+            ops.bilinear(acc[t], self.f_ld, B, self.gh, self.gw, f, h4, w4, out_f32=up[t], out_split=ups.rows_view(t * M4, M4))
         ph = [f"heads.{t}." for t in self.tasks]
         z = _e(T, M4, f, device=dev)
         _grouped([(ups, W[ph[t] + "mt_proj.0.weight"], dict(M=M4, N=f, K=f, bias=self.P_(ph[t] + "mt_proj.0.bias"), out_f32=z[t],
                                                             conv=(B, h4, w4, 3, 1), a_row_offset=t * M4)) for t in range(T)])
         z2s = Split(T * M4, f, dev, ns)
-        bn = [self._bn_fwd(z[t], ph[t] + "mt_proj.1", ACT_GELU, _rows_view(z2s, t * M4, M4)) for t in range(T)]
+        bn = [self._bn_fwd(z[t], ph[t] + "mt_proj.1", ACT_GELU, z2s.rows_view(t * M4, M4)) for t in range(T)]
         out, n_outs = {}, []
         for t, name in enumerate(self.tasks):
             n_out = self.P_(ph[t] + "linear_pred.weight").shape[0]
@@ -477,10 +489,9 @@ class TrainStep:
         ops.split_rows(dX, dXp, rows=Mp, cols=C, in_group=P, src_group=N, src_offset=T)
         dXpT = ops.transpose_planes(dXp, R=Mp, Ccols=C)
         colsT = ops.im2col_patch_t(cx["img"], self.patch, self.ns)
-        gW = self.G_(bbp + "patch_embed.proj.weight").reshape(C, -1)
-        self._gemm(dXpT, colsT, M=C, N=gW.shape[1], K=Mp, residual=gW, out_f32=gW)
-        ops.colsum(dX, self.G_(bbp + "patch_embed.proj.bias"), accumulate=True, rows=Mp, in_group=P, src_group=N,
-                   src_offset=T)
+        pe = bbp + "patch_embed.proj."
+        self._lin_bwd(dX, None, [(self.G_(pe + "weight").reshape(C, -1), self.G_(pe + "bias"), None)], M=Mp, N=C,
+                      K=colsT.rows, dyT=dXpT, aT=colsT, dy_rows=(P, N, T))
         self._bucket_ready(None)
         if self.comm is not None:                       # the communication stream rejoins (required when the step is captured)
             torch.cuda.current_stream(self.dev).wait_stream(self.comm)
@@ -499,8 +510,8 @@ class TrainStep:
             g = grad_out[name].to(dev, torch.float32).contiguous()
             dy = _e(M4, n_out, device=dev)
             ops.bilinear_bwd(g, nchw=True, B=B, h=h4, w=w4, Cdim=n_out, H2=oh, W2=ow, dx=dy)
-            self._lin_bwd(dy, _rows_view(hc["z2s"], t * M4, M4), ph[t] + "linear_pred.weight", M=M4, N=n_out, K=f,
-                          dx_out=dz2[t])
+            self._lin_bwd(dy, hc["z2s"].rows_view(t * M4, M4), [self._wb(ph[t] + "linear_pred")], M=M4, N=n_out, K=f,
+                          dx=dz2[t])
         dz = _e(T, M4, f, device=dev)
         for t in range(T):
             self._bn_bwd(hc["z"][t], dz2[t], ph[t] + "mt_proj.1", ACT_GELU, *hc["bn"][t], dx=dz[t])
@@ -511,48 +522,24 @@ class TrainStep:
 
     def _conv3_bwd_group(self, dy, x32, prefixes, B, h, w, Cin, Cout):
         """3x3 convs (pad 1) of len(prefixes) tasks stacked by rows: dy fp32 [T*Mx, Cout], inputs x32 fp32 [T*Mx, Cin] ->
-        dx fp32 [T*Mx, Cin]; dW (one grouped GEMM over the transposed im2col operand), db."""
+        dx fp32 [T*Mx, Cin]; dW and db as the linear adjoint over the transposed im2col operand."""
         Tn, Mx, dev, ns = len(prefixes), B * h * w, self.dev, self.ns
         dyT = Split(Tn * Cout, Mx, dev, ns)
         ops.transpose_split(dy, dyT, B=Tn, L=Mx, Cdim=Cout)
         x9T = ops.im2col3x3_t(x32, B=Tn * B, H=h, W=w, Cdim=Cin, nsplit=ns)              # [Cin*9, Tn*Mx]: task t = columns t*Mx ..
-        gWs = [self.G_(p + ".weight").reshape(Cout, Cin * 9) for p in prefixes]
+        items = [(self.G_(p + ".weight").reshape(Cout, Cin * 9), self.G_(p + ".bias"), None) for p in prefixes]
         if Mx % 8 == 0:
-            _grouped([(dyT, x9T, dict(M=Cout, N=Cin * 9, K=Mx, a_row_offset=t * Cout, w_col_offset=t * Mx, residual=gWs[t],
-                                      out_f32=gWs[t])) for t in range(Tn)])
-        else:                                             # column offsets must stay 16-byte aligned for TMA
-            for t in range(Tn):
+            self._lin_bwd(dy, None, items, M=Mx, N=Cout, K=Cin * 9, dyT=dyT, aT=x9T)
+        else:                                             # column offsets must stay 16-byte aligned for TMA: one task at a time
+            for t, it in enumerate(items):
                 xt = ops.im2col3x3_t(x32[t * Mx:(t + 1) * Mx], B=B, H=h, W=w, Cdim=Cin, nsplit=ns)
-                self._gemm(dyT, xt, M=Cout, N=Cin * 9, K=Mx, a_row_offset=t * Cout, residual=gWs[t], out_f32=gWs[t])
-        for t, p in enumerate(prefixes):
-            ops.colsum(dy, self.G_(p + ".bias"), accumulate=True, rows=Mx, in_group=Mx, src_group=Mx, src_offset=t * Mx)
+                self._lin_bwd(dy, None, [it], M=Mx, N=Cout, K=Cin * 9, dyT=dyT.rows_view(t * Cout, Cout), aT=xt,
+                              dy_rows=(Mx, Mx, t * Mx))
         dys = self._S(dy)
         dx = _e(Tn * Mx, Cin, device=dev)
         _grouped([(dys, self.WT[p + ".weight"], dict(M=Mx, N=Cin, K=Cout, out_f32=dx[t * Mx:(t + 1) * Mx],
                                                      conv=(B, h, w, 3, 1), a_row_offset=t * Mx)) for t, p in enumerate(prefixes)])
         return dx
-
-    def _lin_bwd_group(self, dy, a_s, items, *, M, N, K, dyT=None, dy_s=None, need_dx=True):
-        """T problems Y_t = A_t W_t^T + b_t stacked by rows: dy fp32 [T*M, N] (any row stride), a_s Split [T*M, K];
-        items[t] = (gW view [N, K], bias-gradient view or None, key of W_t in self.WT). dW / db accumulate; returns
-        (dA fp32 [T*M, K] or None, dyT, dy_s) -- the transposed / split dY can be shared by a second call on the same dY."""
-        Tn, dev, ns = len(items), self.dev, self.ns
-        if dyT is None:
-            dyT = Split(Tn * N, M, dev, ns)
-            ops.transpose_split(dy, dyT, B=Tn, L=M, Cdim=N)
-        aT = ops.transpose_planes(a_s, B=Tn, R=M, Ccols=K)
-        _grouped([(dyT, aT, dict(M=N, N=K, K=M, a_row_offset=t * N, w_row_offset=t * K, residual=it[0], out_f32=it[0]))
-                  for t, it in enumerate(items)])
-        for t, it in enumerate(items):
-            if it[1] is not None:
-                ops.colsum(dy, it[1], accumulate=True, rows=M, in_group=M, src_group=M, src_offset=t * M)
-        dx = None
-        if need_dx:
-            dy_s = self._S(dy) if dy_s is None else dy_s
-            dx = _e(Tn * M, K, device=dev)
-            _grouped([(dy_s, self.WT[it[2]], dict(M=M, N=K, K=N, a_row_offset=t * M, out_f32=dx[t * M:(t + 1) * M]))
-                      for t, it in enumerate(items)])
-        return dx, dyT, dy_s
 
     def _level_bwd(self, lv, dacc, dXsrc, B):
         """Adjoint of _level_fwd: dacc [T, B*P, f_ld] (the same for every level: acc is their sum) -> dXsrc (+=), the logit
@@ -585,25 +572,22 @@ class TrainStep:
         else:
             dF = dacc
         pf = [f"{bbp}fea_fuse.{il}.{t}." for t in self.tasks]
-        G, Pb = self.G_, (lambda n: self.G_(n))
+        G = self.G_
         dFv = dF.view(T * Mp, self.f_ld)[:, :f]
-        dy2, _, _ = self._lin_bwd_group(dFv, lv["y2s"], [(G(p + "4.weight").reshape(f, f), G(p + "4.bias"), p + "4.weight") for p in pf],
-                                        M=Mp, N=f, K=f)
+        dy2 = self._lin_bwd(dFv, lv["y2s"], [self._wb(p + "4") for p in pf], M=Mp, N=f, K=f)[0]
         dy1 = _e(T, Mp, f, device=dev)
         for t in range(T):
             self._bn_bwd(lv["y1"][t], dy2[t * Mp:(t + 1) * Mp], pf[t] + "2", ACT_GELU, *lv["bn"][t], dx=dy1[t])
         dy0 = self._conv3_bwd_group(dy1.view(T * Mp, f), lv["y0"].view(T * Mp, f), [p + "1" for p in pf], B, self.gh, self.gw, f, f)
         g0 = [G(p + "0.weight").reshape(f, 2 * e) for p in pf]
-        ds, dyT, dy0s = self._lin_bwd_group(dy0, lv["s_s"], [(g0[t][:, :e], G(pf[t] + "0.bias"), pf[t] + "0.weight#s")
-                                                             for t in range(T)], M=Mp, N=f, K=e)
-        dc, _, _ = self._lin_bwd_group(dy0, lv["c_s"], [(g0[t][:, e:], None, pf[t] + "0.weight#c") for t in range(T)],
-                                       M=Mp, N=f, K=e, dyT=dyT, dy_s=dy0s)
-        ps = [f"{bbp}fea_decode_spa.{il}.{t}.0." for t in self.tasks]
-        pcn = [f"{bbp}fea_decode_chan.{il}.{t}.0." for t in self.tasks]
-        dys, _, _ = self._lin_bwd_group(ds, lv["ys"], [(G(p + "weight").reshape(e, C), G(p + "bias"), p + "weight") for p in ps],
-                                        M=Mp, N=e, K=C)
-        dyc, _, _ = self._lin_bwd_group(dc, lv["yc"], [(G(p + "weight").reshape(e, C), G(p + "bias"), p + "weight") for p in pcn],
-                                        M=Mp, N=e, K=C)
+        ds, dyT, dy0s = self._lin_bwd(dy0, lv["s_s"], [(g0[t][:, :e], G(pf[t] + "0.bias"), pf[t] + "0.weight#s")
+                                                       for t in range(T)], M=Mp, N=f, K=e)
+        dc = self._lin_bwd(dy0, lv["c_s"], [(g0[t][:, e:], None, pf[t] + "0.weight#c") for t in range(T)], M=Mp, N=f, K=e,
+                           dyT=dyT, dy_s=dy0s)[0]
+        dys = self._lin_bwd(ds, lv["ys"], [self._wb(f"{bbp}fea_decode_spa.{il}.{t}.0") for t in self.tasks], M=Mp, N=e,
+                            K=C)[0]
+        dyc = self._lin_bwd(dc, lv["yc"], [self._wb(f"{bbp}fea_decode_chan.{il}.{t}.0") for t in self.tasks], M=Mp, N=e,
+                            K=C)[0]
         for t in range(T):
             ops.gate_bwd(lv["Xsrc"], N, T, logits, rc, t, dys[t * Mp:(t + 1) * Mp], dyc[t * Mp:(t + 1) * Mp], dXsrc, d_logits,
                          d_rc, B=B, T=T, N=N, H=H, Cdim=C, gh=self.gh, gw=self.gw, nh=self.nh, nw=self.nw)
@@ -623,10 +607,10 @@ class TrainStep:
         else:
             dm = dX2
         a = ops.act_split(bc["pre"], ACT_GELU, nsplit=ns)
-        da = self._lin_bwd(dm, a, b + "mlp.fc2.weight", M=M, N=C, K=bc["pre"].shape[1])
+        da = self._lin_bwd(dm, a, [self._wb(b + "mlp.fc2")], M=M, N=C, K=bc["pre"].shape[1])[0]
         del a
         ops.act_bwd(bc["pre"], da, ACT_GELU, da)
-        dh = self._lin_bwd(da, bc["h"], b + "mlp.fc1.weight", M=M, N=bc["pre"].shape[1], K=C)
+        dh = self._lin_bwd(da, bc["h"], [self._wb(b + "mlp.fc1")], M=M, N=bc["pre"].shape[1], K=C)[0]
         del da
         dX1 = dX2                                                     # residual path; LN2's input gradient is added to it
         ops.layernorm_bwd(bc["X1"], dh, self.P_(b + "norm2.weight"), eps, dX1, self.G_(b + "norm2.weight"),
@@ -641,15 +625,9 @@ class TrainStep:
         # token_trans1 (prompt rows of o): o_p += cp W1^T + b1
         dop = Split(B * T, C, dev, ns)
         ops.split_rows(do, dop, rows=B * T, cols=C, in_group=T, src_group=N, src_offset=0)
-        n1 = b + "attn.token_trans1.weight"
         dopT = ops.transpose_planes(dop, R=B * T, Ccols=C)
-        cpT = ops.transpose_planes(bc["cps"], R=B * T, Ccols=P)
-        g1 = self.G_(n1)
-        self._gemm(dopT, cpT, M=C, N=P, K=B * T, residual=g1, out_f32=g1)
-        ops.colsum(do, self.G_(b + "attn.token_trans1.bias"), accumulate=True, rows=B * T, in_group=T, src_group=N,
-                   src_offset=0)
-        dcp = _e(B * T, P, device=dev)
-        self._gemm(dop, self.WT[n1], M=B * T, N=P, K=C, out_f32=dcp)
+        dcp = self._lin_bwd(do, bc["cps"], [self._wb(b + "attn.token_trans1")], M=B * T, N=C, K=P, dyT=dopT, dy_s=dop,
+                            dy_rows=(T, N, 0))[0]
         # raw channel logits
         if bc["d_rc"] is not None:
             dcp2 = _e(B * T, P, device=dev)
@@ -657,25 +635,21 @@ class TrainStep:
                                 nh=self.nh, nw=self.nw)
             ops.axpy_rows(dcp, dcp2, None, dcp)
         # token_trans: cp = pn Wt^T + bt (pn = prompt rows of xn)
-        n0 = b + "attn.token_trans.weight"
+        tt = b + "attn.token_trans."
         dcps = self._S(dcp)
         dcpT = Split(P, B * T, dev, ns, zero=(B * T) % 8 != 0)
         ops.transpose_split(dcp, dcpT, B=1, L=B * T, Cdim=P)
         pnT = ops.transpose_planes(bc["xn"], B=B, R=T, Ccols=C, in_batch_rows=N, side_by_side=True)   # [C, B*T]
-        g0 = self.G_(n0)
-        self._gemm(dcpT, pnT, M=P, N=C, K=B * T, residual=g0, out_f32=g0)
-        ops.colsum(dcp, self.G_(b + "attn.token_trans.bias"), accumulate=True)
-        bstep = max(1, 128 // T)
-        for b0 in range(0, B, bstep):
-            nb = min(bstep, B - b0)
-            self._gemm(dcps, self.WT[n0], M=nb * T, N=C, K=P, a_row_offset=b0 * T, residual=dxn, out_f32=dxn,
-                     regroup=(T, N, b0 * N))
+        self._lin_bwd(dcp, None, [(self.G_(tt + "weight"), self.G_(tt + "bias"), None)], M=B * T, N=P, K=C, dyT=dcpT, aT=pnT)
+        for b0, nb in prompt_row_chunks(B, T):       # the data gradient is scattered to the prompt rows of dxn, by chunks
+            self._gemm(dcps, self.WT[tt + "weight"], M=nb * T, N=C, K=P, a_row_offset=b0 * T, residual=dxn, out_f32=dxn,
+                       regroup=(T, N, b0 * N))
         # proj
-        dao = self._lin_bwd(do, bc["ao"], b + "attn.proj.weight", M=M, N=C, K=C)
+        dao = self._lin_bwd(do, bc["ao"], [self._wb(b + "attn.proj")], M=M, N=C, K=C)[0]
         # attention
         dqkv = self._attn_bwd(bc, dao, B)
         # qkv
-        self._lin_bwd(dqkv, bc["xn"], b + "attn.qkv.weight", M=M, N=3 * C, K=C, dx_residual=dxn, dx_out=dxn)
+        self._lin_bwd(dqkv, bc["xn"], [self._wb(b + "attn.qkv")], M=M, N=3 * C, K=C, dx=dxn, accumulate_dx=True)
         # LN1
         dX = dX1
         ops.layernorm_bwd(bc["X"], dxn, self.P_(b + "norm1.weight"), eps, dX, self.G_(b + "norm1.weight"),
@@ -909,13 +883,6 @@ class TrainStep:
         params = [p for _, p in self.model.named_parameters()]
         outs = _StepFn.apply(self, images, *params)
         return {t: o for t, o in zip(self.tasks, outs)}
-
-
-def _rows_view(sp, r0, n):
-    """Rows [r0, r0 + n) of a Split as a Split (shares storage)."""
-    v = Split.__new__(Split)
-    v.buf, v.rows, v.cols, v.ld, v.nsplit = sp.buf[:, r0:r0 + n], n, sp.cols, sp.ld, sp.nsplit
-    return v
 
 
 def _grouped(calls, limit=32):

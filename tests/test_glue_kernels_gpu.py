@@ -72,9 +72,7 @@ def test_gate_split(both, cuda_dev):
         ys = [ops.Split(B * P, C, cuda_dev) for _ in range(T)]
         yc = [ops.Split(B * P, C, cuda_dev) for _ in range(T)]
         big = torch.zeros(T, 2, 2, B * P, C, dtype=torch.bfloat16, device=cuda_dev)      # [task][ys|yc][plane]
-        y0, c0 = ops.Split.__new__(ops.Split), ops.Split.__new__(ops.Split)
-        for sp, j in ((y0, 0), (c0, 1)):
-            sp.rows, sp.cols, sp.ld, sp.nsplit, sp.buf = B * P, C, C, 2, big[0, j]
+        y0, c0 = ops.Split.from_planes(big[0, 0], C), ops.Split.from_planes(big[0, 1], C)
         ops.gate_split(x, N, T, lg, rc, 0, y0, c0, B=B, T=T, N=N, H=H, Cdim=C, gh=gh, gw=gw, nh=nh, nw=nh, ntasks=T,
                        task_stride=big.stride(0))
         torch.cuda.synchronize()

@@ -60,11 +60,7 @@ def _split(dev, g, rows, cols, r, nsplit=2, ld=None, pad=0.0, lo_zero=False):
 
 
 def _to(sp, dev):
-    ops = _ops()
-    out = ops.Split.__new__(ops.Split)
-    out.rows, out.cols, out.ld, out.nsplit = sp.rows, sp.cols, sp.ld, sp.nsplit
-    out.buf = sp.buf.to(dev, copy=True)
-    return out
+    return _ops().Split.from_planes(sp.buf.to(dev, copy=True), sp.cols)
 
 
 def _conv_weight(dev, g, Cout, Cin, ks, r, nsplit=2):
