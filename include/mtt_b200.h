@@ -256,6 +256,55 @@ int mtt_bilinear_postproc(const float* in, int64_t ld_in, int32_t B, int32_t h, 
 int mtt_preprocess_image(const uint8_t* img, int32_t B, int32_t h, int32_t w, int32_t bgr, const float* mean3,
                          const float* std3, float* out, int32_t H, int32_t W, mtt_stream_t stream);
 
+/* Training-time augmentation of the reference (TP/utils/common_config.py:96-121, TP/data/transforms.py) over a ragged
+ * batch of raw samples, in at most three launches. train != 0: RandomScaling(0.5, 2) -> RandomCrop(crop,
+ * cat_max_ratio 0.75) -> RandomHorizontalFlip -> PhotoMetricDistortion -> Normalize -> PadImage(crop) ->
+ * AddIgnoreRegions -> ToTensor, with every random draw given in the sample records; train == 0: the validation chain
+ * Normalize -> PadImage -> AddIgnoreRegions -> ToTensor (records carry scale 1 and no crop; H x W is the padded size,
+ * max(raw, test size), equal for every sample).
+ * `samples` (device) holds B mtt_augment_sample records; `data` (device) the raw float32 HWC arrays they point into:
+ * image [h,w,3] with integer values 0..255, label maps [h,w,1] (semseg, human_parts, sal, edge, depth) or [h,w,3]
+ * (normals); semseg holds integer labels (255 = ignore). Outputs: image_out fp32 [B,3,H,W], task_out[t] fp32
+ * [B,C,H,W]. workspace: mtt_augment_workspace_bytes(B) bytes (4-byte aligned): per (sample, candidate) flags
+ * (bit 0 cat_max_ratio test passed, bit 1 human_parts crop is all 0 / 255), then the chosen candidate per sample
+ * (int32, -1 = no crop). Bit-exact against the reference on the labels and on every stage after the uint8 cast of the
+ * image; the cv2 rules restated are listed in oracle/augment_ref.py. */
+#define MTT_AUG_MAX_TASKS 7
+#define MTT_AUG_CANDIDATES 11
+enum mtt_aug_task {
+  MTT_AUG_SEMSEG = 0, MTT_AUG_HUMAN_PARTS = 1, MTT_AUG_SAL = 2, MTT_AUG_EDGE = 3, MTT_AUG_NORMALS = 4, MTT_AUG_DEPTH = 5
+};
+typedef struct {
+  int64_t off[1 + MTT_AUG_MAX_TASKS]; /* float offsets into data: the image, then task t's map */
+  double lin_y, lin_x;                /* h / sh, w / sw: the INTER_LINEAR source step */
+  double nn_y, nn_x;                  /* 1 / (sh / h), 1 / (sw / w): the INTER_NEAREST source step */
+  int32_t h, w, sh, sw;               /* raw and scaled size (scaled = raw when scale == 1) */
+  int32_t scaled;                     /* scale != 1: depth is divided by depth_scale = float32(scale) */
+  float depth_scale;
+  int32_t ncand;                      /* 0: the scaled size equals the crop size (no crop), else MTT_AUG_CANDIDATES */
+  int32_t cand[MTT_AUG_CANDIDATES][2]; /* crop offsets (y, x) */
+  int32_t flip;
+  int32_t bright_on, f_mode, contrast_on, sat_on, hue_on;
+  float beta, alpha, sat_alpha;
+  int32_t hue_delta;
+} mtt_augment_sample;
+typedef struct {
+  const void* samples;
+  const float* data;
+  int32_t B, H, W;
+  int32_t train;
+  int32_t crop_h, crop_w; /* train: the crop size (= H, W) */
+  int32_t ntasks;
+  int32_t task_kind[MTT_AUG_MAX_TASKS]; /* mtt_aug_task, each at most once; train needs semseg */
+  float* task_out[MTT_AUG_MAX_TASKS];
+  float* image_out;
+  float mean[3], std[3];
+  void* workspace;
+  size_t workspace_bytes;
+} mtt_augment_desc;
+size_t mtt_augment_workspace_bytes(int32_t B);
+int mtt_augment(const mtt_augment_desc* d, mtt_stream_t stream);
+
 /* Sum of up to three bilinearly resized NHWC fp32 sources written once as a split tensor [B*H2*W2, ld_bf]:
  * InvPT's multi-scale aggregation of the three stages' per-task maps (IP invpt.py:528-539), in the
  * reference's accumulation order, without read-modify-write passes over the full-resolution map. */

@@ -68,6 +68,31 @@ class BilinearSrc(C.Structure):
                 ("batch_rows", C.c_int64), ("row_offset", C.c_int64)]
 
 
+AUG_MAX_TASKS, AUG_CANDIDATES = 7, 11
+AUG_TASK_KIND = {"semseg": 0, "human_parts": 1, "sal": 2, "edge": 3, "normals": 4, "depth": 5}
+
+
+class AugmentSample(C.Structure):
+    _fields_ = [("off", C.c_int64 * (1 + AUG_MAX_TASKS)),
+                ("lin_y", C.c_double), ("lin_x", C.c_double), ("nn_y", C.c_double), ("nn_x", C.c_double),
+                ("h", C.c_int32), ("w", C.c_int32), ("sh", C.c_int32), ("sw", C.c_int32),
+                ("scaled", C.c_int32), ("depth_scale", C.c_float),
+                ("ncand", C.c_int32), ("cand", C.c_int32 * (2 * AUG_CANDIDATES)),
+                ("flip", C.c_int32),
+                ("bright_on", C.c_int32), ("f_mode", C.c_int32), ("contrast_on", C.c_int32), ("sat_on", C.c_int32),
+                ("hue_on", C.c_int32),
+                ("beta", C.c_float), ("alpha", C.c_float), ("sat_alpha", C.c_float), ("hue_delta", C.c_int32)]
+
+
+class AugmentDesc(C.Structure):
+    _fields_ = [("samples", C.c_void_p), ("data", C.c_void_p),
+                ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("train", C.c_int32),
+                ("crop_h", C.c_int32), ("crop_w", C.c_int32), ("ntasks", C.c_int32),
+                ("task_kind", C.c_int32 * AUG_MAX_TASKS), ("task_out", C.c_void_p * AUG_MAX_TASKS),
+                ("image_out", C.c_void_p), ("mean", C.c_float * 3), ("std", C.c_float * 3),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+
+
 # name -> (restype, argtypes); every symbol include/mtt_b200.h declares
 _i64, _i32, _f32, _vp = C.c_int64, C.c_int32, C.c_float, C.c_void_p
 SYMBOLS = {
@@ -102,7 +127,9 @@ SYMBOLS = {
     "mtt_preprocess_image": (C.c_int, [_vp, _i32, _i32, _i32, _i32, C.POINTER(C.c_float), C.POINTER(C.c_float), _vp,
                                        _i32, _i32, _vp]),
     "mtt_bilinear_postproc": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
-    "mtt_bilinear_sum3": (C.c_int, [C.POINTER(BilinearSrc), _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
+    "mtt_augment_workspace_bytes": (C.c_size_t, [_i32]),
+    "mtt_augment": (C.c_int, [C.POINTER(AugmentDesc), _vp]),
+    "mtt_bilinear_sum3": (C.c_int,[C.POINTER(BilinearSrc), _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
     "mtt_split_rows": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _i64, _i64, _i32, _vp]),
     "mtt_layernorm_seg": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i32, _vp, _vp, _f32, _vp, _i64, _vp,
                                     _vp, _i64, _i64, _i64, _i32, _vp]),

@@ -418,6 +418,31 @@ def preprocess_image(img_u8, out_hw, *, bgr=True, mean=IMAGENET_MEAN, std=IMAGEN
     return out
 
 
+def augment_workspace_bytes(B):
+    return int(_L.load().mtt_augment_workspace_bytes(int(B)))
+
+
+def augment(samples, data, *, B, H, W, train, crop_hw, tasks, task_out, image_out, workspace,
+            mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """The reference's train (train=True) or validation transform chain over a packed ragged batch
+    (mtt_augment): samples = device bytes of B mtt_augment_sample records, data = device float32 raw arrays;
+    tasks = task names (keys of lib.AUG_TASK_KIND) in the records' offset order, task_out / image_out = fp32 NCHW
+    outputs; workspace = int32 device tensor of augment_workspace_bytes(B) bytes."""
+    d = _L.AugmentDesc()
+    d.samples, d.data = samples.data_ptr(), data.data_ptr()
+    d.B, d.H, d.W, d.train = int(B), int(H), int(W), int(bool(train))
+    d.crop_h, d.crop_w = (int(crop_hw[0]), int(crop_hw[1])) if train else (0, 0)
+    d.ntasks = len(tasks)
+    for i, (t, o) in enumerate(zip(tasks, task_out)):
+        d.task_kind[i] = _L.AUG_TASK_KIND[t]
+        d.task_out[i] = o.data_ptr()
+    d.image_out = image_out.data_ptr()
+    for c in range(3):
+        d.mean[c], d.std[c] = mean[c], std[c]
+    d.workspace, d.workspace_bytes = workspace.data_ptr(), workspace.numel() * workspace.element_size()
+    _L.check(_L.load().mtt_augment(C.byref(d), _stream()), "mtt_augment")
+
+
 def bilinear_sum3(srcs, out, *, B, Cdim, H2, W2):
     """out (Split [B*H2*W2, C]) = sum_i bilinear(src_i -> H2 x W2); srcs: list of up to three
     (tensor fp32 [rows, ld], h, w, batch_rows, row_offset)."""
