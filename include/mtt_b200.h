@@ -305,6 +305,58 @@ typedef struct {
 size_t mtt_augment_workspace_bytes(int32_t B);
 int mtt_augment(const mtt_augment_desc* d, mtt_stream_t stream);
 
+/* Predictions -> uint8 images, for the reference's prediction export (save_model_pred_for_one_task,
+ * TP/evaluation/evaluate_utils.py:69-151, IP/evaluation/evaluate_utils.py:69-105) and inference visualisation
+ * (vis_pred_for_one_task, TP/utils/visualization_utils.py:80-199). One descriptor per task; all (task, image) pairs of
+ * a call are rendered by one pre-pass launch (JET min / max, all-ignore label flags) and one main launch:
+ *   source   LOGITS fp32 [B,C,h,w] (the wrapper's output), bilinearly resized to out_h x out_w (F.interpolate,
+ *            align_corners=False; no resize when equal) and post-processed with get_output kind `postproc` (0 argmax,
+ *            1 edge, 2 sal, 3 normals, 4 depth: the per-pixel code of mtt_bilinear_postproc); or a get_output map as
+ *            predict() returns it, not resized: CLASS int64 [B,h,w], MAP fp32 [B,h,w,C] with C = 1 or 3;
+ *   crop     per image (y0, x0, h, w) inside the out_h x out_w map, or inside out_size[i] when given (LOGITS: a
+ *            resize target per image); host arrays, read at enqueue;
+ *   encode   U8: astype(np.uint8) of a scalar map; CLASS: the class id as uint8, through `table` (256 ids, optional);
+ *            PALETTE_BGR: RGB palette[class] stored B, G, R; NORMALS_BGR: the three channels truncated, stored B, G, R;
+ *            JET: (v - min) / (max - min) * 255 in float32 over the image's crop, truncated, then the BGR `table`.
+ *            Truncation is numpy's float32 -> uint8 cast on x86-64: the low byte of the int32 truncation, where NaN
+ *            and out-of-range values give INT32_MIN; so a constant map (max == min, 0 / 0 = NaN) is JET index 0.
+ *   store    uint8 at out + offset[i] (host array of byte offsets), [h,w] or HWC [h,w,3].
+ * `label` (optional, device fp32 [B,label_numel]) sets flags[i] (device int32 [B]) to 1 when every value of image i's
+ * label equals ignore_index (the reference's `len(label.unique()) == 1 and label.unique() == ignore` skip rule).
+ * Tables are device data. workspace: mtt_render_workspace_bytes(n, max B) bytes, 4-byte aligned; the call zeroes it
+ * with cudaMemsetAsync. At most MTT_RENDER_MAX_TASKS descriptors and MTT_RENDER_MAX_IMAGES (task, image) pairs per
+ * call. Rejected: unknown kinds, a get_output kind the channel count cannot take, an encoding the source cannot take,
+ * a palette shorter than the class count C, a crop outside the map, an offset outside out_bytes. */
+#define MTT_RENDER_MAX_TASKS 8
+#define MTT_RENDER_MAX_IMAGES 96
+enum mtt_render_src { MTT_RENDER_SRC_LOGITS = 0, MTT_RENDER_SRC_CLASS = 1, MTT_RENDER_SRC_MAP = 2 };
+enum mtt_render_encode {
+  MTT_RENDER_U8 = 0, MTT_RENDER_CLASS = 1, MTT_RENDER_PALETTE_BGR = 2, MTT_RENDER_NORMALS_BGR = 3, MTT_RENDER_JET = 4
+};
+typedef struct {
+  int32_t src_kind;       /* mtt_render_src */
+  const void* src;        /* device */
+  int32_t B, C, h, w;     /* source geometry; C: logit channels, MAP channels, or the class count of a CLASS map */
+  int32_t out_h, out_w;   /* LOGITS: resize target; CLASS / MAP: h, w */
+  int32_t postproc;       /* LOGITS: get_output kind 0..4; ignored otherwise */
+  int32_t encode;         /* mtt_render_encode */
+  const uint8_t* table;   /* device: palette [table_len][3] RGB, class-id table [table_len >= 256], JET [256][3] BGR */
+  int32_t table_len;
+  const int32_t* crop;    /* host [B][4]: y0, x0, h, w */
+  const int64_t* offset;  /* host [B]: byte offset of each image in out */
+  const int32_t* out_size; /* host [B][2], optional (LOGITS): per-image resize target instead of out_h x out_w */
+  uint8_t* out;           /* device */
+  int64_t out_bytes;
+  const float* label;     /* device, optional */
+  int64_t label_numel;    /* per image */
+  float ignore_index;
+  int32_t* flags;         /* device int32 [B]; required with label */
+} mtt_render_desc;
+size_t mtt_render_workspace_bytes(int32_t n_tasks, int32_t B);
+int mtt_render(const mtt_render_desc* d, int32_t n, void* workspace, mtt_stream_t stream);
+/* cv2.applyColorMap(np.arange(256, dtype=np.uint8), cv2.COLORMAP_JET): 256 BGR triples (host memory). */
+const uint8_t* mtt_render_jet_bgr(void);
+
 /* Sum of up to three bilinearly resized NHWC fp32 sources written once as a split tensor [B*H2*W2, ld_bf]:
  * InvPT's multi-scale aggregation of the three stages' per-task maps (IP invpt.py:528-539), in the
  * reference's accumulation order, without read-modify-write passes over the full-resolution map. */

@@ -6,6 +6,7 @@
 #include <stdlib.h>
 
 #include "host_common.h"
+#include "postproc.cuh"
 #include "ptx.cuh"
 
 namespace mtt {
@@ -206,16 +207,8 @@ ctr_mix_kernel(const float* __restrict__ F, const float* __restrict__ w, float* 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Bilinear resize, align_corners = False (ATen upsample_bilinear2d semantics; reference calls at
-// taskprompter.py:420, taskprompter_wrapper.py:35).  NHWC fp32 in; NHWC (fp32 and/or split) or NCHW out.
-__device__ __forceinline__ void bilin_coord(int d, float scale, int in_size, int& i0, int& i1, float& l1) {
-  float s = scale * (d + 0.5f) - 0.5f;
-  if (s < 0.f) s = 0.f;
-  i0 = (int)s;
-  if (i0 > in_size - 1) i0 = in_size - 1;
-  i1 = i0 + (i0 < in_size - 1 ? 1 : 0);
-  l1 = s - (float)i0;
-}
+// Bilinear resize, align_corners = False (bilin_coord, postproc.cuh).  NHWC fp32 in; NHWC (fp32 and/or split) or
+// NCHW out.
 
 // One warp per (run of up to kBilinRun consecutive output pixels of one output row, chunk of 64 * NCH channels). A lane
 // owns NCH channel pairs (c, c + 64, ...) and walks the run keeping the four corner values of each pair in registers:
@@ -500,12 +493,8 @@ bilinear_sum3_kernel(BilinSrc s0, BilinSrc s1, BilinSrc s2, int B, int C, int H2
 }
 
 // Bilinear resize to the output size fused with the reference's prediction post-processing
-// (get_output, TP/utils/utils.py:27-63): the full-resolution fp32 logits are never written.
-//   kind 0: argmax over channels -> int64 [B,H2,W2]        (semseg, human_parts; first maximum wins, like torch.max)
-//   kind 1: 255 * sigmoid(x)     -> fp32  [B,H2,W2]        (edge)
-//   kind 2: 255 * softmax(x)[1]  -> fp32  [B,H2,W2]        (sal, 2 channels)
-//   kind 3: (x/||x|| + 1)*255/2  -> fp32  [B,H2,W2,3]      (normals; F.normalize eps 1e-12)
-//   kind 4: max(x, 0)            -> fp32  [B,H2,W2,1]      (depth)
+// (get_output_pixel, postproc.cuh): the full-resolution fp32 logits are never written. Kind 0 writes int64 [B,H2,W2],
+// kinds 1, 2 and 4 fp32 [B,H2,W2] (depth: [B,H2,W2,1]), kind 3 fp32 [B,H2,W2,3].
 __global__ void __launch_bounds__(256)
 bilinear_postproc_kernel(const float* __restrict__ in, long long ld_in, int B, int h, int w, int C, int H2, int W2,
                          float sy, float sx, int kind, long long* __restrict__ out_i64, float* __restrict__ out_f32) {
@@ -523,33 +512,15 @@ bilinear_postproc_kernel(const float* __restrict__ in, long long ld_in, int B, i
   const float* p11 = ib + ((long long)y1 * w + x1) * ld_in;
   const float hy = 1.f - ly, hx = 1.f - lx;
   auto val = [&](int c) { return hy * (hx * p00[c] + lx * p01[c]) + ly * (hx * p10[c] + lx * p11[c]); };
-  if (kind == 0) {
-    float best = val(0);
-    int bi = 0;
-    for (int c = 1; c < C; ++c) {
-      const float v = val(c);
-      if (v > best) {
-        best = v;
-        bi = c;
-      }
-    }
-    out_i64[opix] = bi;
-  } else if (kind == 1) {
-    out_f32[opix] = 255.f * (1.f / (1.f + expf(-val(0))));
-  } else if (kind == 2) {
-    const float a = val(0), c1 = val(1);
-    const float m = fmaxf(a, c1);
-    const float e0 = expf(a - m), e1 = expf(c1 - m);
-    out_f32[opix] = e1 / (e0 + e1) * 255.f;
-  } else if (kind == 3) {
-    const float a = val(0), c1 = val(1), c2 = val(2);
-    const float n = fmaxf(sqrtf(a * a + c1 * c1 + c2 * c2), 1e-12f);
-    out_f32[opix * 3 + 0] = (a / n + 1.f) * 255.f / 2.f;
-    out_f32[opix * 3 + 1] = (c1 / n + 1.f) * 255.f / 2.f;
-    out_f32[opix * 3 + 2] = (c2 / n + 1.f) * 255.f / 2.f;
-  } else {
-    out_f32[opix] = fmaxf(val(0), 0.f);
-  }
+  struct Sink {
+    long long* i64;
+    float* f32;
+    long long opix;
+    __device__ void cls(int c) { i64[opix] = c; }
+    __device__ void f1(float v) { f32[opix] = v; }
+    __device__ void ch(int c, float v) { f32[opix * 3 + c] = v; }
+  } sink{out_i64, out_f32, opix};
+  get_output_pixel(kind, C, val, sink);
 }
 
 }  // namespace mtt

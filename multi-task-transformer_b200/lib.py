@@ -93,6 +93,22 @@ class AugmentDesc(C.Structure):
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
 
 
+RENDER_MAX_TASKS, RENDER_MAX_IMAGES = 8, 96
+RENDER_SRC_LOGITS, RENDER_SRC_CLASS, RENDER_SRC_MAP = 0, 1, 2
+RENDER_U8, RENDER_CLASS, RENDER_PALETTE_BGR, RENDER_NORMALS_BGR, RENDER_JET = 0, 1, 2, 3, 4
+
+
+class RenderDesc(C.Structure):
+    _fields_ = [("src_kind", C.c_int32), ("src", C.c_void_p),
+                ("B", C.c_int32), ("C", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
+                ("out_h", C.c_int32), ("out_w", C.c_int32), ("postproc", C.c_int32), ("encode", C.c_int32),
+                ("table", C.c_void_p), ("table_len", C.c_int32),
+                ("crop", C.POINTER(C.c_int32)), ("offset", C.POINTER(C.c_int64)), ("out_size", C.POINTER(C.c_int32)),
+                ("out", C.c_void_p), ("out_bytes", C.c_int64),
+                ("label", C.c_void_p), ("label_numel", C.c_int64), ("ignore_index", C.c_float),
+                ("flags", C.c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/mtt_b200.h declares
 _i64, _i32, _f32, _vp = C.c_int64, C.c_int32, C.c_float, C.c_void_p
 SYMBOLS = {
@@ -129,6 +145,9 @@ SYMBOLS = {
     "mtt_bilinear_postproc": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "mtt_augment_workspace_bytes": (C.c_size_t, [_i32]),
     "mtt_augment": (C.c_int, [C.POINTER(AugmentDesc), _vp]),
+    "mtt_render_workspace_bytes": (C.c_size_t, [_i32, _i32]),
+    "mtt_render": (C.c_int, [C.POINTER(RenderDesc), _i32, _vp, _vp]),
+    "mtt_render_jet_bgr": (C.POINTER(C.c_uint8), []),
     "mtt_bilinear_sum3": (C.c_int,[C.POINTER(BilinearSrc), _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
     "mtt_split_rows": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _vp, _vp, _i64, _i64, _i32, _vp]),
     "mtt_layernorm_seg": (C.c_int, [_vp, _i64, _i64, _i64, _i64, _i64, _i32, _vp, _vp, _f32, _vp, _i64, _vp,

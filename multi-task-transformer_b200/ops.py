@@ -443,6 +443,95 @@ def augment(samples, data, *, B, H, W, train, crop_hw, tasks, task_out, image_ou
     _L.check(_L.load().mtt_augment(C.byref(d), _stream()), "mtt_augment")
 
 
+RENDER_ENCODE = {"u8": _L.RENDER_U8, "class": _L.RENDER_CLASS, "palette_bgr": _L.RENDER_PALETTE_BGR,
+                 "normals_bgr": _L.RENDER_NORMALS_BGR, "jet": _L.RENDER_JET}
+RENDER_CHANNELS = {"u8": 1, "class": 1, "palette_bgr": 3, "normals_bgr": 3, "jet": 3}
+
+
+def render_workspace_bytes(n_tasks, B):
+    return int(_L.load().mtt_render_workspace_bytes(int(n_tasks), int(B)))
+
+
+def _render_source(what, src, postproc, n_classes):
+    """(source kind, C, h, w) of a render source, or ValueError: fp32 NCHW logits when postproc (a get_output kind) is
+    given, else predict()'s int64 [B,h,w] class map or fp32 [B,h,w] / [B,h,w,1] / [B,h,w,3] map."""
+    if postproc is not None:
+        if src.dtype != torch.float32 or src.dim() != 4:
+            raise ValueError(f"{what}: logits must be fp32 [B,C,h,w], got {src.dtype} {tuple(src.shape)}")
+        return _L.RENDER_SRC_LOGITS, int(src.shape[1]), int(src.shape[2]), int(src.shape[3])
+    if src.dtype == torch.int64 and src.dim() == 3:
+        return _L.RENDER_SRC_CLASS, int(n_classes or 1), int(src.shape[1]), int(src.shape[2])
+    if src.dtype == torch.float32 and (src.dim() == 3 or (src.dim() == 4 and src.shape[3] in (1, 3))):
+        return _L.RENDER_SRC_MAP, int(src.shape[3]) if src.dim() == 4 else 1, int(src.shape[1]), int(src.shape[2])
+    raise ValueError(f"{what}: a get_output map must be int64 [B,h,w] or fp32 [B,h,w(,1|3)], got {src.dtype} "
+                     f"{tuple(src.shape)}")
+
+
+def render(tasks, workspace):
+    """Predictions -> uint8 images (mtt_render): one pre-pass and one main launch for all tasks. `tasks` is a list of
+    dicts, one per task, with
+      src       fp32 NCHW logits (with postproc = get_output kind, ops.POSTPROC_KIND) or a get_output map (postproc
+                None; n_classes = the class count of an int64 map, for the palette check)
+      out_hw    the resize target of logits (default: the logits' size); out_sizes: one (h, w) per image instead
+      encode    a key of RENDER_ENCODE; table: uint8 CUDA tensor (palette [N,3] RGB, id table [256], JET [256,3])
+      crops     host int [B,4] (y0, x0, h, w); offsets: host int [B] byte offsets into out (uint8 CUDA tensor)
+      label     optional fp32 CUDA tensor [B,...] with flags (int32 CUDA [B]) and ignore_index: the all-ignore flag.
+    Every tensor is checked (dtype, shape, contiguity, device) before anything is launched."""
+    import numpy as np
+    if not 0 < len(tasks) <= _L.RENDER_MAX_TASKS:
+        raise ValueError(f"render: 1..{_L.RENDER_MAX_TASKS} tasks per call, got {len(tasks)}")
+    descs = (_L.RenderDesc * len(tasks))()
+    keep = []
+    for i, t in enumerate(tasks):
+        what = f"render(task {i})"
+        src, post = t["src"], t.get("postproc")
+        kind, Cs, h, w = _render_source(what, src, post, t.get("n_classes"))
+        B = int(src.shape[0])
+        enc = t["encode"]
+        if enc not in RENDER_ENCODE:
+            raise ValueError(f"{what}: encode must be one of {sorted(RENDER_ENCODE)}, got {enc!r}")
+        out, table, label, flags = t["out"], t.get("table"), t.get("label"), t.get("flags")
+        tensors = [src, out] + [x for x in (table, label, flags) if x is not None]
+        if not all(isinstance(x, torch.Tensor) and x.is_cuda for x in tensors):
+            raise RuntimeError(f"{what}: every tensor must be a CUDA tensor (there is no CPU path)")
+        if len({x.device for x in tensors + [workspace]}) != 1:
+            raise RuntimeError(f"{what}: tensors on different devices")
+        if not all(x.is_contiguous() for x in tensors):
+            raise ValueError(f"{what}: tensors must be contiguous")
+        if out.dtype != torch.uint8 or (table is not None and table.dtype != torch.uint8):
+            raise ValueError(f"{what}: out and table must be uint8")
+        if label is not None and (label.dtype != torch.float32 or label.shape[0] != B or flags is None or
+                                  flags.dtype != torch.int32 or flags.numel() < B):
+            raise ValueError(f"{what}: label must be fp32 [B,...] with int32 flags [B]")
+        crops = np.ascontiguousarray(np.asarray(t["crops"], dtype=np.int32).reshape(-1, 4))
+        offs = np.ascontiguousarray(np.asarray(t["offsets"], dtype=np.int64).reshape(-1))
+        if crops.shape[0] != B or offs.shape[0] != B:
+            raise ValueError(f"{what}: {B} images need {B} crops and offsets, got {crops.shape[0]} / {offs.shape[0]}")
+        oh, ow = t.get("out_hw") or (h, w)
+        sizes = t.get("out_sizes")
+        if sizes is not None:
+            sizes = np.ascontiguousarray(np.asarray(sizes, dtype=np.int32).reshape(B, 2))
+        keep += [crops, offs, sizes]
+        d = descs[i]
+        d.src_kind, d.src, d.B, d.C, d.h, d.w = kind, src.data_ptr(), B, Cs, h, w
+        d.out_h, d.out_w = int(oh), int(ow)
+        d.postproc = -1 if post is None else int(post)
+        d.encode = RENDER_ENCODE[enc]
+        d.table = table.data_ptr() if table is not None else None
+        d.table_len = (table.shape[0] if table is not None else 0)
+        d.crop = crops.ctypes.data_as(C.POINTER(C.c_int32))
+        d.offset = offs.ctypes.data_as(C.POINTER(C.c_int64))
+        d.out_size = sizes.ctypes.data_as(C.POINTER(C.c_int32)) if sizes is not None else None
+        d.out, d.out_bytes = out.data_ptr(), out.numel()
+        d.label = label.data_ptr() if label is not None else None
+        d.label_numel = label[0].numel() if label is not None else 0
+        d.ignore_index = float(t.get("ignore_index", 255))
+        d.flags = flags.data_ptr() if flags is not None else None
+    if workspace.numel() * workspace.element_size() < render_workspace_bytes(1, sum(d.B for d in descs)):
+        raise ValueError("render: workspace smaller than render_workspace_bytes")
+    _L.check(_L.load().mtt_render(descs, len(tasks), _ptr(workspace), _stream()), "mtt_render")
+
+
 def bilinear_sum3(srcs, out, *, B, Cdim, H2, W2):
     """out (Split [B*H2*W2, C]) = sum_i bilinear(src_i -> H2 x W2); srcs: list of up to three
     (tensor fp32 [rows, ld], h, w, batch_rows, row_offset)."""
