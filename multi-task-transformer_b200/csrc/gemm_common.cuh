@@ -33,8 +33,7 @@ struct GemmParams {
   long long ldo_bf;
   int in_group, out_group, out_offset;
   int out_row_stride;  // >= 1: stride of the in-group row index (see mtt_gemm_desc)
-  int vec_ok;
-  int vec32_ok;  // every epilogue pointer / stride allows 32-byte accesses
+  int vec_ok;  // every epilogue pointer is 16-byte aligned, ldr and ldo_f32 % 4 == 0, ldo_bf % 8 == 0
   int a_groups_per_tile;  // >0: A rows are gathered in groups through a rank-3 tensor map
   int debug;              // profiling aid (env MTT_GEMM_DEBUG): bit0 = skip TMA loads, bit1 = skip the epilogue,
                           // bit2 = run the epilogue without its global stores
@@ -129,71 +128,68 @@ __device__ __forceinline__ RowInfo row_info(const GemmParams& p, int ms, int row
   return r;
 }
 
-// ---- fused epilogue for the two adjacent columns n, n + 1 of one row: bias, activation, residual, fp32 and
-// split-bf16 stores. The kernel reads the bias (epilogue_bias2) and the residual (staged in shared memory) before it
-// calls epilogue_store2, which only computes and stores.
-__device__ __forceinline__ float2 epilogue_bias2(const GemmParams& p, int n) {  // zero where absent or n >= N
-  float2 b = make_float2(0.f, 0.f);
-  if (!p.bias || n >= p.N) return b;
-  if (n + 1 < p.N && p.vec_ok) {  // n is even: 8-byte fp32 pairs are aligned
-    b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-  } else {
-    b.x = __ldg(p.bias + n);
-    if (n + 1 < p.N) b.y = __ldg(p.bias + n + 1);
-  }
+// ---- fused epilogue: bias, activation, residual, fp32 and split-bf16 stores of four adjacent columns n .. n + 3 of one
+// row. The variant is fixed at compile time: ACT (mtt_act) and OUT (which outputs the descriptor has); bias and
+// residual stay warp-uniform runtime flags. The kernel reads the bias (epilogue_bias4) once per chunk and the residual
+// from shared memory before it calls epilogue_store4, which only computes and stores. `full`: all four columns lie
+// inside N and the vector accesses are aligned (vec_ok: 16-byte fp32 and 8-byte bf16 groups, since n % 4 == 0);
+// otherwise the columns inside N are written one by one.
+enum { kOutF32 = 1, kOutSplit = 2, kOutBoth = 3 };
+
+__device__ __forceinline__ float4 epilogue_bias4(const GemmParams& p, int n, bool full) {  // zero where absent or >= N
+  float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (!p.bias) return b;
+  if (full) return __ldg(reinterpret_cast<const float4*>(p.bias + n));
+  if (n < p.N) b.x = __ldg(p.bias + n);
+  if (n + 1 < p.N) b.y = __ldg(p.bias + n + 1);
+  if (n + 2 < p.N) b.z = __ldg(p.bias + n + 2);
+  if (n + 3 < p.N) b.w = __ldg(p.bias + n + 3);
   return b;
 }
-// mo: output row (RowInfo::mo); b, r: bias and residual of the pair
-__device__ __forceinline__ void epilogue_store2(const GemmParams& p, float v0, float v1, int n, long long mo, float2 b,
-                                                float2 r) {
-  if (n >= p.N) return;
-  const bool two = n + 1 < p.N;
-  const bool vec = two && p.vec_ok;  // n is even: 8-byte fp32 pairs and 4-byte bf16 pairs are aligned
-  if (p.bias) {
-    v0 += b.x;
-    v1 += b.y;
-  }
-  if (p.act == MTT_ACT_GELU) {
-    v0 = gelu_erf(v0);
-    v1 = gelu_erf(v1);
-  } else if (p.act == MTT_ACT_RELU) {
-    v0 = fmaxf(v0, 0.f);
-    v1 = fmaxf(v1, 0.f);
-  }
-  if (p.residual) {
-    v0 += r.x;
-    v1 += r.y;
-  }
+// one element: bias add, activation, residual add, in that order (the adds only where the descriptor has the operand)
+template <int ACT>
+__device__ __forceinline__ float epilogue_op(float v, float b, float r, bool bias, bool res) {
+  if (bias) v += b;
+  if (ACT == MTT_ACT_GELU) v = gelu_erf(v);
+  if (ACT == MTT_ACT_RELU) v = fmaxf(v, 0.f);
+  if (res) v += r;
+  return v;
+}
+// v: the four accumulator values, b / r: their bias and residual; of / ob: element offsets of column n of the output
+// row in out_f32 / out_hi and out_lo
+template <int ACT, int OUT>
+__device__ __forceinline__ void epilogue_store4(const GemmParams& p, float4 v, float4 b, float4 r, long long of,
+                                                long long ob, int n, bool full) {
+  const bool bias = p.bias != nullptr, res = p.residual != nullptr;
+  v.x = epilogue_op<ACT>(v.x, b.x, r.x, bias, res);
+  v.y = epilogue_op<ACT>(v.y, b.y, r.y, bias, res);
+  v.z = epilogue_op<ACT>(v.z, b.z, r.z, bias, res);
+  v.w = epilogue_op<ACT>(v.w, b.w, r.w, bias, res);
   if (p.debug & 4) {  // profiling aid: the arithmetic runs, the global stores do not
-    asm volatile("" ::"f"(v0), "f"(v1));
+    asm volatile("" ::"f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w));
     return;
   }
-  if (p.out_f32) {
-    float* op = p.out_f32 + mo * p.ldo_f32 + n;
-    if (vec) {
-      *reinterpret_cast<float2*>(op) = make_float2(v0, v1);
-    } else {
-      op[0] = v0;
-      if (two) op[1] = v1;
+  if (full) {
+    if (OUT & kOutF32) *reinterpret_cast<float4*>(p.out_f32 + of) = v;
+    if (OUT & kOutSplit) {
+      uint2 h, l;
+      split_pack2(v.x, v.y, h.x, l.x);
+      split_pack2(v.z, v.w, h.y, l.y);
+      *reinterpret_cast<uint2*>(p.out_hi + ob) = h;
+      if (p.out_lo) *reinterpret_cast<uint2*>(p.out_lo + ob) = l;
     }
+    return;
   }
-  if (p.out_hi) {
-    const long long o = mo * p.ldo_bf + n;
-    if (vec) {
-      uint32_t h, l;
-      split_pack2(v0, v1, h, l);
-      *reinterpret_cast<uint32_t*>(p.out_hi + o) = h;
-      if (p.out_lo) *reinterpret_cast<uint32_t*>(p.out_lo + o) = l;
-    } else {
+  const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    if (n + k >= p.N) break;
+    if (OUT & kOutF32) p.out_f32[of + k] = e[k];
+    if (OUT & kOutSplit) {
       __nv_bfloat16 h, l;
-      split_bf16(v0, h, l);
-      p.out_hi[o] = h;
-      if (p.out_lo) p.out_lo[o] = l;
-      if (two) {
-        split_bf16(v1, h, l);
-        p.out_hi[o + 1] = h;
-        if (p.out_lo) p.out_lo[o + 1] = l;
-      }
+      split_bf16(e[k], h, l);
+      p.out_hi[ob + k] = h;
+      if (p.out_lo) p.out_lo[ob + k] = l;
     }
   }
 }

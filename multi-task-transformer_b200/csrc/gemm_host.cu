@@ -35,6 +35,8 @@ int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensor
   if (!d->a_hi || !d->b_hi || (d->nsplit == 2 && (!d->a_lo || !d->b_lo)))
     return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm: missing operand plane");
   if (!d->out_f32 && !d->out_hi) return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm: no output");
+  if (d->act != MTT_ACT_NONE && d->act != MTT_ACT_GELU && d->act != MTT_ACT_RELU)
+    return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm: act=%d (0 none, 1 GELU, 2 ReLU)", d->act);
   if (d->lda % 8 || d->ldb % 8)
     return set_error(MTT_ERR_MISALIGNED, "mtt_gemm: lda=%lld ldb=%lld must be multiples of 8",
                      (long long)d->lda, (long long)d->ldb);
@@ -77,12 +79,6 @@ int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensor
   if (d->residual && (!al16(d->residual) || d->ldr % 4)) p.vec_ok = 0;
   if (d->out_f32 && (!al16(d->out_f32) || d->ldo_f32 % 4)) p.vec_ok = 0;
   if (d->out_hi && (!al16(d->out_hi) || d->ldo_bf % 8 || (p.out_lo && !al16(p.out_lo)))) p.vec_ok = 0;
-  auto al32 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 31) == 0; };
-  p.vec32_ok = p.vec_ok;
-  if (d->bias && !al32(d->bias)) p.vec32_ok = 0;
-  if (d->residual && (!al32(d->residual) || d->ldr % 8)) p.vec32_ok = 0;
-  if (d->out_f32 && (!al32(d->out_f32) || d->ldo_f32 % 8)) p.vec32_ok = 0;
-  if (d->out_hi && (!al32(d->out_hi) || d->ldo_bf % 16 || (p.out_lo && !al32(p.out_lo)))) p.vec32_ok = 0;
 
   int rc;
   const int ksq = (d->mode == 1) ? d->ksize * d->ksize : 1;

@@ -23,7 +23,7 @@
 
 namespace mtt {
 
-constexpr int kEpiCols = 32;  // columns per staged epilogue chunk: 16 lanes per row, two rows per pass
+constexpr int kEpiCols = 32;  // columns per staged epilogue chunk: 8 lanes per row, four rows per pass
 
 template <int NSPLIT, int BN>
 struct GemmCfg {
@@ -110,8 +110,9 @@ __device__ __forceinline__ unsigned int sk_flag_peek(const unsigned int* f) {
 }
 
 // The kernel body, shared by the single-problem kernel (GROUPED = false: `maps` holds one set of four tensor maps)
-// and the grouped one (GROUPED = true: one set per problem, tile -> (problem, tile) through grp).
-template <int NSPLIT, int BN, bool GROUPED, bool SK>
+// and the grouped one (GROUPED = true: one set per problem, tile -> (problem, tile) through grp). ACT and OUT fix the
+// epilogue variant (epilogue_store4).
+template <int NSPLIT, int BN, bool GROUPED, bool SK, int ACT, int OUT>
 __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const GemmParams& p, const GemmGroup* grp) {
   static_assert(!SK || (BN == 256 && !GROUPED), "stream-K: single-problem kernel with 256-wide tiles only");
   using Cfg = GemmCfg<NSPLIT, BN>;
@@ -208,11 +209,12 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
     const uint32_t a_frag_off = a_off + (uint32_t)lrow * 128;
     const int a_chunk = lane >> 4, a_xor = lane & 7;
     const int wrow0 = cw * 64 + (warp & 3) * 16;  // the warp's first row in the tile
-    float* ebuf = reinterpret_cast<float*>(smem + ST * Cfg::kStageBytes + 256) + ew * 2 * 16 * kEpiCols;
-    float* rbuf = ebuf + 16 * kEpiCols;  // the residual of the chunk in ebuf
-    // the residual row of each of the warp's 16 rows (-1: the row is not written), set when a piece starts; kept in
-    // shared memory, since the registers beside the 128 x 256 tile's accumulator are few
-    long long* rmap = reinterpret_cast<long long*>(smem + ST * Cfg::kStageBytes + 256 + Cfg::kEpiBufBytes) + ew * 16;
+    // the warp's epilogue buffers, as shared addresses: ebuf, a 16 x kEpiCols fp32 chunk of the accumulator
+    const uint32_t ebuf = smem_u32(smem + ST * Cfg::kStageBytes + 256) + ew * (2 * 16 * kEpiCols * 4);
+    const uint32_t rbuf = ebuf + 16 * kEpiCols * 4;  // the residual of the chunk in ebuf
+    // the residual row of each of the warp's 16 rows (8 bytes each, -1: the row is not written), set when a piece
+    // starts; kept in shared memory, since the registers beside the 128 x 256 tile's accumulator are few
+    const uint32_t rmap = smem_u32(smem + ST * Cfg::kStageBytes + 256 + Cfg::kEpiBufBytes) + ew * 16 * 8;
     // Copies the residual of rows [8 half, 8 half + 8) of the warp's 16, columns [n0, n0 + kEpiCols), to rbuf as one
     // cp.async group. Lane l copies columns 4 (l % 8) .. 4 (l % 8) + 3 of rows 8 half + l / 8 and 8 half + l / 8 + 4;
     // what lies outside the problem is zero-filled.
@@ -221,8 +223,8 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
 #pragma unroll
       for (int k = 0; k < 2; ++k) {
         const int r = 8 * half + (lane >> 3) + 4 * k;
-        const long long m = rmap[r];
-        const uint32_t dst = smem_u32(rbuf + r * kEpiCols + 4 * (lane & 7));
+        const long long m = ld_shared_s64(rmap + 8 * r);
+        const uint32_t dst = rbuf + (r * kEpiCols + 4 * (lane & 7)) * 4;
         const float* src = res + (m >= 0 ? m * p.ldr + n : 0);
         if (p.vec_ok) {  // residual and ldr 16-byte aligned, n % 4 == 0
           const int cols = m >= 0 ? min(max(p.N - n, 0), 4) : 0;
@@ -266,7 +268,7 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
         if (res && !(SK && kbeg > 0) && !(p.debug & 2)) {  // a stream-K contribution has no epilogue
           if (lane < 16) {
             const RowInfo ri = row_info(p, mt, wrow0 + lane);
-            rmap[lane] = ri.ok ? ri.mr : -1;
+            st_shared_s64(rmap + 8 * lane, ri.ok ? ri.mr : -1);
           }
           __syncwarp();
           res_issue(res, nt * BN, 0);
@@ -388,29 +390,45 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
       const GemmParams& pq = GROUPED ? pg : p;  // single problem: read straight from the kernel parameters
       // The warp's 16 x BN slice goes out in 16 x kEpiCols chunks through its shared-memory buffer, with no global
       // load on the per-row path:
-      //   * row map: lane l holds the output row of the warp's row l % 16 (row_info, once per piece), which the row
-      //     loop reads with a shuffle; the residual rows are in rmap;
-      //   * the bias pair is read once per chunk, while the fragment is written to ebuf;
+      //   * lane l writes rows 4 q + l / 8 (q = 0..3) of every chunk, columns 4 (l % 8) .. 4 (l % 8) + 3. The element
+      //     offsets of the warp's 16 output rows in out_f32 and in out_hi / out_lo are computed once per piece from the
+      //     row map (row_info), lane l holding those of row l % 16; a pass reads its row's with a shuffle and adds its
+      //     column (four rows of offsets per lane would not fit beside the 128 x 256 tile's accumulator). The residual
+      //     rows are in rmap;
+      //   * the bias of the lane's four columns is read once per chunk, while the fragment is written to ebuf;
       //   * the chunk's residual is in rbuf (cp.async: the first chunk's was issued when the piece started, each half
-      //     of a later chunk's while the same half of the chunk before it is stored).
-      // The fragment is written with unrolled stores (acc needs compile-time indices, hence the branch per chunk in
-      // the rolled chunk loop), then 8 passes store two rows each, lanes 0-15 on row 2 q and 16-31 on row 2 q + 1, two
-      // columns per lane, one contiguous 128-byte fp32 segment per row. Unrolling the whole epilogue over the fragment
-      // made it tens of thousands of instructions long and bound by instruction fetch. Columns are XOR-swizzled by row
-      // in 8-column groups, so both sides of ebuf are free of bank conflicts.
+      //     of a later chunk's while the same half of the chunk before it is stored). res_issue makes lane l copy the
+      //     residual of the same rows and columns it stores.
+      // The fragment is written with unrolled 8-byte shared stores (acc needs compile-time indices, hence the branch
+      // per chunk in the rolled chunk loop), then 4 passes store four rows each, 8 lanes per row, four columns per
+      // lane: one contiguous 128-byte fp32 segment (64 bytes per bf16 plane) per row. Unrolling the whole epilogue
+      // over the fragment made it tens of thousands of instructions long and bound by instruction fetch. Columns are
+      // XOR-swizzled by row in 8-column groups, so both sides of ebuf are free of bank conflicts: a half-warp of the
+      // fragment stores covers rows 4 k .. 4 k + 3 and 8 columns of each, a quarter-warp of the 16-byte pass reads one
+      // row.
       // The residual may be the output itself (x += f(x)): a chunk's residual is in shared memory before any store of
       // that chunk, and the copy of chunk c + 1 overlaps only the stores of chunk c, whose columns are disjoint from it.
-      long long mo_map;
+      const int lr = lane >> 3, c4 = 4 * (lane & 7);  // this lane's rows (4 q + lr) and first column in a chunk
+      long long of_map, ob_map;  // row lane % 16 of the warp: element offsets of its column 0 in out_f32 / out_hi, out_lo
+      int rows_ok = 0;           // bit q: row 4 q + lr is written
       {
         const RowInfo ri = row_info(p, mt, wrow0 + (lane & 15));
-        mo_map = ri.ok ? ri.mo : -1;
+        of_map = ri.mo * pq.ldo_f32;
+        ob_map = ri.mo * pq.ldo_bf;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) rows_ok |= (__shfl_sync(0xffffffffu, (int)ri.ok, 4 * q + lr) & 1) << q;
       }
-      const int hr = lane >> 4, cl = 2 * (lane & 15);  // this lane's row in a pass (2 q + hr) and column in a chunk
+      // fragment stores: row (lane / 4) + 8 h, columns 8 j + col0 + {0, 1} at 8-column group j ^ (row % 4)
+      const uint32_t e_wr = ebuf + ((lane >> 2) * kEpiCols + col0) * 4, e_sw = ((lane >> 2) & 3) * 32;
+      // pass reads: row 4 q + lr (row % 4 == lr), columns c4 .. c4 + 3 at their swizzled place
+      const uint32_t e_rd = ebuf + (lr * kEpiCols + (c4 ^ (lr << 3))) * 4;
+      const uint32_t r_rd = rbuf + (lr * kEpiCols + c4) * 4;
       constexpr int kChunks = BN / kEpiCols;
 #pragma unroll 1
       for (int c = 0; c < kChunks; ++c) {
-        const int n0 = nt * BN + c * kEpiCols, n = n0 + cl;
-        const float2 b = epilogue_bias2(pq, n);
+        const int n0 = nt * BN + c * kEpiCols, n = n0 + c4;
+        const bool full = pq.vec_ok && n + 4 <= pq.N;
+        const float4 b = epilogue_bias4(pq, n, full);
 #pragma unroll
         for (int cc = 0; cc < kChunks; ++cc) {
           if (cc != c) continue;
@@ -418,21 +436,19 @@ __device__ __forceinline__ void gemm_tc_body(const CUtensorMap (*maps)[4], const
           for (int j = 0; j < kEpiCols / 8; ++j)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              const int r = (lane >> 2) + 8 * h, i = cc * (kEpiCols / 8) + j;
-              *reinterpret_cast<float2*>(ebuf + r * kEpiCols + ((8 * j + col0) ^ ((r & 3) << 3))) =
-                  make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
+              const int i = cc * (kEpiCols / 8) + j;
+              st_shared_v2(e_wr + h * 8 * kEpiCols * 4 + ((j * 32) ^ e_sw), acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
             }
         }
-        // rows [8 half, 8 half + 8) of the chunk: 4 passes
+        // rows [8 half, 8 half + 8) of the chunk: passes q = 2 half, 2 half + 1
         auto store_rows = [&](int half) {
-#pragma unroll
-          for (int q = 4 * half; q < 4 * half + 4; ++q) {
-            const int r = 2 * q + hr;
-            const long long mo = __shfl_sync(0xffffffffu, mo_map, r);
-            const float2 v = *reinterpret_cast<const float2*>(ebuf + r * kEpiCols + (cl ^ ((r & 3) << 3)));
-            const float2 rv = pq.residual ? *reinterpret_cast<const float2*>(rbuf + r * kEpiCols + cl)
-                                          : make_float2(0.f, 0.f);
-            if (mo >= 0) epilogue_store2(pq, v.x, v.y, n, mo, b, rv);
+#pragma unroll 1
+          for (int q = 2 * half; q < 2 * half + 2; ++q) {
+            const float4 v = ld_shared_v4(e_rd + q * 4 * kEpiCols * 4);
+            const float4 rv = pq.residual ? ld_shared_v4(r_rd + q * 4 * kEpiCols * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
+            const long long of = (OUT & kOutF32) ? __shfl_sync(0xffffffffu, of_map, 4 * q + lr) + n : 0;
+            const long long ob = (OUT & kOutSplit) ? __shfl_sync(0xffffffffu, ob_map, 4 * q + lr) + n : 0;
+            if (rows_ok & (1 << q)) epilogue_store4<ACT, OUT>(pq, v, b, rv, of, ob, n, full);
           }
         };
         // The residual arrives in two groups per chunk, rows 0-7 and rows 8-15; each half of rbuf is refilled with the
@@ -463,17 +479,17 @@ struct GemmMaps1 {
   CUtensorMap m[1][4];
 };
 
-template <int NSPLIT, int BN, bool SK>
+template <int NSPLIT, int BN, bool SK, int ACT, int OUT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_kernel(const __grid_constant__ GemmMaps1 maps, const GemmParams p) {
-  gemm_tc_body<NSPLIT, BN, false, SK>(maps.m, p, nullptr);
+  gemm_tc_body<NSPLIT, BN, false, SK, ACT, OUT>(maps.m, p, nullptr);
 }
 
-template <int NSPLIT, int BN>
+template <int NSPLIT, int BN, int ACT, int OUT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_tc_grouped_kernel(const __grid_constant__ GemmGroupMaps maps, const __grid_constant__ GemmGroup grp,
                        const GemmParams p) {
-  gemm_tc_body<NSPLIT, BN, true, false>(maps.m, p, &grp);
+  gemm_tc_body<NSPLIT, BN, true, false, ACT, OUT>(maps.m, p, &grp);
 }
 
 // the dynamic shared-memory opt-in is per device and per kernel instantiation
@@ -487,29 +503,57 @@ static int opt_in_smem(Kernel k, uint32_t bytes, bool (&done)[kMaxDevices], cons
   return MTT_OK;
 }
 
+// The epilogue variant of a descriptor, as compile-time constants: its activation (gemm_prepare admits none, GELU and
+// ReLU) and which outputs it has (at least one). f(EpiKind<ACT, OUT>{}) launches that variant's kernel.
+template <int ACT_, int OUT_>
+struct EpiKind {
+  static constexpr int ACT = ACT_, OUT = OUT_;
+};
+template <int ACT, typename F>
+static int with_epilogue_out(const GemmParams& p, F&& f) {
+  if (!p.out_hi) return f(EpiKind<ACT, kOutF32>{});
+  if (!p.out_f32) return f(EpiKind<ACT, kOutSplit>{});
+  return f(EpiKind<ACT, kOutBoth>{});
+}
+template <typename F>
+static int with_epilogue(const GemmParams& p, F&& f) {
+  switch (p.act) {
+    case MTT_ACT_NONE: return with_epilogue_out<MTT_ACT_NONE>(p, f);
+    case MTT_ACT_GELU: return with_epilogue_out<MTT_ACT_GELU>(p, f);
+    case MTT_ACT_RELU: return with_epilogue_out<MTT_ACT_RELU>(p, f);
+  }
+  return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm: no kernel for act=%d", p.act);
+}
+
 template <int NSPLIT, int BN, bool SK>
 static int launch_gemm(const CUtensorMap* maps, const GemmParams& p, int grid, cudaStream_t stream) {
   using Cfg = GemmCfg<NSPLIT, BN>;
-  static bool attr_set[kMaxDevices] = {};
-  int rc = opt_in_smem(gemm_tc_kernel<NSPLIT, BN, SK>, Cfg::kSmemBytes, attr_set, "gemm");
-  if (rc) return rc;
   GemmMaps1 gm;
   for (int i = 0; i < 4; ++i) gm.m[0][i] = maps[i];
-  gemm_tc_kernel<NSPLIT, BN, SK><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(gm, p);
-  return check_launch(SK ? "mtt_gemm(stream-K)" : "mtt_gemm");
+  return with_epilogue(p, [&](auto e) {
+    using E = decltype(e);
+    static bool attr_set[kMaxDevices] = {};
+    int rc = opt_in_smem(gemm_tc_kernel<NSPLIT, BN, SK, E::ACT, E::OUT>, Cfg::kSmemBytes, attr_set, "gemm");
+    if (rc) return rc;
+    gemm_tc_kernel<NSPLIT, BN, SK, E::ACT, E::OUT><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(gm, p);
+    return check_launch(SK ? "mtt_gemm(stream-K)" : "mtt_gemm");
+  });
 }
 
 template <int NSPLIT, int BN>
 static int launch_gemm_grouped(const GemmGroupMaps& gm, const GemmGroup& grp, const GemmParams& p,
                                cudaStream_t stream) {
   using Cfg = GemmCfg<NSPLIT, BN>;
-  static bool attr_set[kMaxDevices] = {};
-  int rc = opt_in_smem(gemm_tc_grouped_kernel<NSPLIT, BN>, Cfg::kSmemBytes, attr_set, "gemm(grouped)");
-  if (rc) return rc;
   const int tiles = grp.tiles_per_problem * grp.count;
   const int grid = tiles < sm_count() ? tiles : sm_count();
-  gemm_tc_grouped_kernel<NSPLIT, BN><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(gm, grp, p);
-  return check_launch("mtt_gemm_grouped");
+  return with_epilogue(p, [&](auto e) {
+    using E = decltype(e);
+    static bool attr_set[kMaxDevices] = {};
+    int rc = opt_in_smem(gemm_tc_grouped_kernel<NSPLIT, BN, E::ACT, E::OUT>, Cfg::kSmemBytes, attr_set, "gemm(grouped)");
+    if (rc) return rc;
+    gemm_tc_grouped_kernel<NSPLIT, BN, E::ACT, E::OUT><<<grid, kGemmThreads, Cfg::kSmemBytes, stream>>>(gm, grp, p);
+    return check_launch("mtt_gemm_grouped");
+  });
 }
 
 int launch_gemm_tiles_grouped(const mtt_gemm_desc* d, int count, int bn, cudaStream_t stream) {
@@ -526,7 +570,6 @@ int launch_gemm_tiles_grouped(const mtt_gemm_desc* d, int count, int bn, cudaStr
       p = pg;
     } else {  // the epilogue's vector width is shared
       p.vec_ok = p.vec_ok && pg.vec_ok;
-      p.vec32_ok = p.vec32_ok && pg.vec32_ok;
     }
     grp.prob[g] = GroupProblem{pg.bias, pg.residual, pg.out_f32, pg.out_hi, pg.out_lo};
   }

@@ -150,6 +150,25 @@ __device__ __forceinline__ void cp_async_ca4(uint32_t dst, const void* src, uint
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+
+// ---------------------------------------------------------------- shared memory through 32-bit shared addresses
+// (a generic pointer into shared memory compiles to LD.E / ST.E, which may alias global memory)
+__device__ __forceinline__ void st_shared_v2(uint32_t a, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory");
+}
+__device__ __forceinline__ float4 ld_shared_v4(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ void st_shared_s64(uint32_t a, long long v) {
+  asm volatile("st.shared.s64 [%0], %1;" ::"r"(a), "l"(v) : "memory");
+}
+__device__ __forceinline__ long long ld_shared_s64(uint32_t a) {
+  long long v;
+  asm volatile("ld.shared.s64 %0, [%1];" : "=l"(v) : "r"(a));
+  return v;
+}
 template <int kPending>
 __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(kPending) : "memory");
