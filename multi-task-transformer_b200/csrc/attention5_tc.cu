@@ -1,12 +1,14 @@
 // Fused multi-head attention, the kernel of mtt_attention (contract in attention_tc.cu:
 // TP/models/transformers/taskprompter.py:204-210, prompt-row raw logits :436-437,:482; IP vit.py:189-193).
 //
-// Warp-specialised wgmma kernel for sm_90a.  Each CTA (288 threads, two CTAs per SM) owns one (batch, head,
-// 128-query tile) item:
-//   * warp 8 = TMA producer: the item's query tile once, then 64-key K and V blocks through two-stage rings;
-//   * warps 0-7 = two consumer warpgroups, 64 query rows each.  Per key block: S = Q K^T as an SS-form wgmma
-//     (m64n64k16, Q and K from shared memory), an online softmax on the accumulator fragment (a row lives in the four
-//     lanes of a quad: max / sum exchange by two shuffles), then P V as an RS-form wgmma that takes P straight
+// Warp-specialised wgmma kernel for sm_90a.  Each CTA (512 threads, one CTA per SM) owns one (batch, head,
+// 192-query tile) item:
+//   * warpgroup 0 = TMA producer (warp 0 issues; the warpgroup gives its registers to the consumers with setmaxnreg):
+//     the item's query tile once, then 64-key K and V blocks through three-stage rings;
+//   * warpgroups 1-3 = consumers, 64 query rows each.  A consumer warpgroup whose rows all lie past N exits at once;
+//     the K / V release barriers count only the warpgroups with rows inside the sequence.  Per key block: S = Q K^T
+//     as an SS-form wgmma (m64n64k16, Q and K from shared memory), an online softmax on the accumulator fragment (a
+//     row lives in the four lanes of a quad: max / sum exchange by two shuffles), then P V as an RS-form wgmma that takes P straight
 //     from registers -- the S accumulator fragment of 16 keys is, element for element, the A fragment of one k16 step --
 //     added to the rescaled O in fp32 (not accumulated inside the tensor core, which truncates);
 //   * split-bf16 parity mode (NSPLIT = 2): every product is hi*hi + hi*lo + lo*hi, P included (split on the fly);
@@ -18,11 +20,15 @@
 
 namespace mtt {
 
-constexpr int kA5Consumers = 256;                // two warpgroups
-constexpr int kA5Threads = kA5Consumers + 32;    // + the TMA warp
-constexpr uint32_t kA5QTile = 128 * 64 * 2;      // one plane of the query tile (16 KB)
-constexpr uint32_t kA5KVTile = 64 * 64 * 2;      // one plane of a 64-key K or V block (8 KB)
-constexpr int kA5Stages = 2;
+// Three consumer warpgroups at 160 registers (parity mode needs O, the block's PV accumulator and the split P
+// fragments live at once: 96 registers before addressing) and a 24-register producer warpgroup fill the register file:
+// 128 * 24 + 384 * 160 = 64512 of 65536.
+constexpr int kA5ConsumerWGs = 3;
+constexpr int kA5Rows = 64 * kA5ConsumerWGs;             // query rows per item
+constexpr int kA5Threads = 128 + 128 * kA5ConsumerWGs;   // producer warpgroup + consumers
+constexpr uint32_t kA5QTile = kA5Rows * 64 * 2;          // one plane of the query tile (24 KB)
+constexpr uint32_t kA5KVTile = 64 * 64 * 2;              // one plane of a 64-key K or V block (8 KB)
+constexpr int kA5Stages = 3;
 
 struct Attn5Params {
   int B, N, H, T;
@@ -33,7 +39,7 @@ struct Attn5Params {
 };
 
 template <int NSPLIT>
-__global__ void __launch_bounds__(kA5Threads, 2)
+__global__ void __launch_bounds__(kA5Threads, 1)
 attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_constant__ CUtensorMap tmq_lo,
                   const __grid_constant__ CUtensorMap tmk_hi, const __grid_constant__ CUtensorMap tmk_lo,
                   const Attn5Params p) {
@@ -54,14 +60,14 @@ attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_const
   const int warp = tid >> 5;
   const int lane = tid & 31;
   const int C = p.H * 64;
-  const int nq = (p.N + 127) / 128;
   const int nkv = (p.N + 63) / 64;
-  const int item = blockIdx.x;
-  const int qt = item % nq;
-  const int h = (item / nq) % p.H;
-  const int b = item / (nq * p.H);
+  // query-tile-major order: the last tile of every (batch, head), the one with rows past N, is dispatched last
+  const int qt = blockIdx.x / (p.B * p.H);
+  const int h = blockIdx.x % p.H;
+  const int b = (blockIdx.x / p.H) % p.B;
+  const int n_act = min(kA5ConsumerWGs, (p.N - qt * kA5Rows + 63) / 64);  // consumer warpgroups with rows < N
 
-  if (tid == kA5Consumers) {
+  if (tid == 0) {
     tma_prefetch_desc(&tmq_hi);
     tma_prefetch_desc(&tmk_hi);
     if (NSPLIT == 2) {
@@ -71,20 +77,22 @@ attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_const
     mbar_init(q_full, 1);
     for (int s = 0; s < kA5Stages; ++s) {
       mbar_init(&k_full[s], 1);
-      mbar_init(&k_empty[s], kA5Consumers / 32);
+      mbar_init(&k_empty[s], 4 * n_act);  // one arrival per active consumer warp
       mbar_init(&v_full[s], 1);
-      mbar_init(&v_empty[s], kA5Consumers / 32);
+      mbar_init(&v_empty[s], 4 * n_act);
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == kA5Consumers / 32) {
-    // ------------------------------------------------------------------ TMA warp (elected lane issues)
+  if (warp < 4) {
+    // ------------------------------------------------------------------ TMA producer (warp 0, elected lane issues)
+    setmaxnreg_dec<24>();
+    if (warp != 0) return;
     if (elect_one()) {
       mbar_arrive_expect_tx(q_full, NSPLIT * kA5QTile);
-      tma_load_3d(sQ, &tmq_hi, q_full, h * 64, qt * 128, b);
-      if (NSPLIT == 2) tma_load_3d(sQ + kA5QTile, &tmq_lo, q_full, h * 64, qt * 128, b);
+      tma_load_3d(sQ, &tmq_hi, q_full, h * 64, qt * kA5Rows, b);
+      if (NSPLIT == 2) tma_load_3d(sQ + kA5QTile, &tmq_lo, q_full, h * 64, qt * kA5Rows, b);
     }
     __syncwarp();
     for (int j = 0; j < nkv; ++j) {
@@ -111,7 +119,9 @@ attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_const
   }
 
   // -------------------------------------------------------------------- consumers
-  const int cw = warp >> 2;                                   // rows [64 cw, 64 cw + 64) of the query tile
+  setmaxnreg_inc<160>();
+  const int cw = (warp >> 2) - 1;                             // rows [64 cw, 64 cw + 64) of the query tile
+  if (cw >= n_act) return;                                    // all rows past N: no MMA, not counted by the barriers
   const int rloc = cw * 64 + (warp & 3) * 16 + (lane >> 2);   // this thread's rows: rloc and rloc + 8
   const int col0 = 2 * (lane & 3);                            // ... and columns col0 + 8 i + {0, 1}
   const uint32_t q_hi = smem_u32(sQ) + (uint32_t)cw * 64 * 128;
@@ -157,7 +167,7 @@ attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_const
     if (p.prompt_logits) {
 #pragma unroll
       for (int hh = 0; hh < 2; ++hh) {
-        const int q_row = qt * 128 + rloc + 8 * hh;
+        const int q_row = qt * kA5Rows + rloc + 8 * hh;
         if (q_row < p.T) {
           float* ex = p.prompt_logits + (((long long)b * p.H + h) * p.T + q_row) * p.N + j * 64;
 #pragma unroll
@@ -203,7 +213,8 @@ attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_const
 
     // ---- O = alpha O + P V: the fragment of keys [16 kk, 16 kk + 16) is the A operand of k-step kk. The block's PV
     // is summed in a fresh accumulator and added to O with round-to-nearest FMAs: the tensor core adds into its
-    // accumulator with truncation, which over many key blocks would bias O towards zero.
+    // accumulator with truncation, which over many key blocks would bias O towards zero. A ragged last block runs all
+    // four k-steps (P is 0 past N, V zero-filled): a divergent exit inside the chain makes ptxas serialise its MMAs.
     uint32_t ph_[4][4], pl_[4][4];
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
@@ -223,7 +234,6 @@ attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_const
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
-      if (kk * 16 >= kn) break;
       const uint64_t vdh = gmma_desc_sw128(v_hi + kk * 2048);  // V rows are keys: MN-major B operand
       wgmma_rs_n64<1>(pvb, ph_[kk], vdh, kk > 0 ? 1 : 0);
       if (NSPLIT == 2) {
@@ -249,7 +259,7 @@ attention5_kernel(const __grid_constant__ CUtensorMap tmq_hi, const __grid_const
     l += __shfl_xor_sync(0xffffffffu, l, 1);
     l += __shfl_xor_sync(0xffffffffu, l, 2);
     const float inv = 1.0f / l;
-    const int q_row = qt * 128 + rloc + 8 * hh;
+    const int q_row = qt * kA5Rows + rloc + 8 * hh;
     if (q_row >= p.N) continue;
     const long long off = ((long long)b * p.N + q_row) * C + h * 64 + col0;
 #pragma unroll
@@ -273,17 +283,17 @@ static int launch_attn5(const CUtensorMap* maps, const Attn5Params& p, cudaStrea
       return set_error(MTT_ERR_LAUNCH, "attention: cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     attr_set[dev_] = true;
   }
-  const int total = ((p.N + 127) / 128) * p.H * p.B;
+  const int total = ((p.N + kA5Rows - 1) / kA5Rows) * p.H * p.B;
   attention5_kernel<NSPLIT><<<total, kA5Threads, smem, stream>>>(maps[0], maps[1], maps[2], maps[3], p);
   return check_launch("mtt_attention");
 }
 
 int launch_attention5(const mtt_attn_desc* d, cudaStream_t stream) {
   const int C = d->H * 64;
-  CUtensorMap maps[4];   // q hi/lo (128-row box), k|v hi/lo (64-row box)
+  CUtensorMap maps[4];   // q hi/lo (kA5Rows-row box), k|v hi/lo (64-row box)
   const uint64_t dims[3] = {(uint64_t)3 * C, (uint64_t)d->N, (uint64_t)d->B};
   const uint64_t str[2] = {(uint64_t)3 * C * 2, (uint64_t)d->N * 3 * C * 2};
-  const uint32_t qbox[3] = {64, 128, 1};
+  const uint32_t qbox[3] = {64, kA5Rows, 1};
   const uint32_t kbox[3] = {64, 64, 1};
   int rc;
   if ((rc = make_tmap_bf16(&maps[0], d->qkv_hi, 3, dims, str, qbox))) return rc;
