@@ -25,6 +25,16 @@ static void pick_conv_tile(int H, int W, int* TW, int* TH) {
   *TH = bth;
 }
 
+// The tensor maps of one split-bf16 operand: the hi plane's in maps[0], the lo plane's in maps[1] (nsplit 1 has no lo
+// plane; maps[1] repeats maps[0]).
+static int make_split_maps(const void* hi, const void* lo, int nsplit, int rank, const uint64_t* dims,
+                           const uint64_t* strides, const uint32_t* box, CUtensorMap* maps) {
+  int rc = make_tmap_bf16(&maps[0], hi, rank, dims, strides, box);
+  if (rc) return rc;
+  if (nsplit == 2) return make_tmap_bf16(&maps[1], lo, rank, dims, strides, box);
+  maps[1] = maps[0];
+  return MTT_OK;
+}
 
 int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensorMap maps[4]) {
   if (!d) return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm: null descriptor");
@@ -103,12 +113,7 @@ int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensor
     const uint64_t dims[3] = {(uint64_t)d->K, (uint64_t)g, (uint64_t)ngroups};
     const uint64_t str[2] = {(uint64_t)d->lda * 2, (uint64_t)d->a_group_stride * d->lda * 2};
     const uint32_t box[3] = {BK, (uint32_t)g, (uint32_t)p.a_groups_per_tile};
-    if ((rc = make_tmap_bf16(&maps[0], d->a_hi, 3, dims, str, box))) return rc;
-    if (d->nsplit == 2) {
-      if ((rc = make_tmap_bf16(&maps[1], d->a_lo, 3, dims, str, box))) return rc;
-    } else {
-      maps[1] = maps[0];
-    }
+    if ((rc = make_split_maps(d->a_hi, d->a_lo, d->nsplit, 3, dims, str, box, &maps[0]))) return rc;
   } else if (d->mode == 0) {
     p.taps = 1;
     p.ksize = 1;
@@ -119,12 +124,7 @@ int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensor
     const uint64_t dims[2] = {(uint64_t)d->K, (uint64_t)d->M};
     const uint64_t str[1] = {(uint64_t)d->lda * 2};
     const uint32_t box[2] = {BK, BM};
-    if ((rc = make_tmap_bf16(&maps[0], d->a_hi, 2, dims, str, box))) return rc;
-    if (d->nsplit == 2) {
-      if ((rc = make_tmap_bf16(&maps[1], d->a_lo, 2, dims, str, box))) return rc;
-    } else {
-      maps[1] = maps[0];
-    }
+    if ((rc = make_split_maps(d->a_hi, d->a_lo, d->nsplit, 2, dims, str, box, &maps[0]))) return rc;
   } else if (d->mode == 1) {
     if (d->B <= 0 || d->H <= 0 || d->W <= 0 || (long long)d->B * d->H * d->W != d->M)
       return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm(conv): B*H*W = %d*%d*%d != M = %d", d->B, d->H,
@@ -148,12 +148,7 @@ int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensor
     const uint64_t str[3] = {(uint64_t)d->lda * 2, (uint64_t)d->W * d->lda * 2,
                              (uint64_t)d->H * d->W * d->lda * 2};
     const uint32_t box[4] = {BK, (uint32_t)p.TW, (uint32_t)p.TH, 1};
-    if ((rc = make_tmap_bf16(&maps[0], d->a_hi, 4, dims, str, box))) return rc;
-    if (d->nsplit == 2) {
-      if ((rc = make_tmap_bf16(&maps[1], d->a_lo, 4, dims, str, box))) return rc;
-    } else {
-      maps[1] = maps[0];
-    }
+    if ((rc = make_split_maps(d->a_hi, d->a_lo, d->nsplit, 4, dims, str, box, &maps[0]))) return rc;
   } else {
     return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm: mode=%d", d->mode);
   }
@@ -165,12 +160,7 @@ int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensor
     const uint64_t dims[2] = {ktot, (uint64_t)d->N};
     const uint64_t str[1] = {(uint64_t)d->ldb * 2};
     const uint32_t box[2] = {BK, (uint32_t)b_box_rows};
-    if ((rc = make_tmap_bf16(&maps[2], d->b_hi, 2, dims, str, box))) return rc;
-    if (d->nsplit == 2) {
-      if ((rc = make_tmap_bf16(&maps[3], d->b_lo, 2, dims, str, box))) return rc;
-    } else {
-      maps[3] = maps[2];
-    }
+    if ((rc = make_split_maps(d->b_hi, d->b_lo, d->nsplit, 2, dims, str, box, &maps[2]))) return rc;
   }
   return MTT_OK;
 }
@@ -178,6 +168,44 @@ int gemm_prepare(const mtt_gemm_desc* d, int b_box_rows, GemmParams& p, CUtensor
 // -1: read MTT_GEMM_VARIANT once; 0 auto, 1 = 128x128 tiles, 2 = 128x256 tiles (stream-K capable), 3 = 128x128 tiles
 // (the number once named a CTA-pair tile shape; it is kept so that existing settings still select a valid kernel)
 static int g_variant = -1;
+
+// Columns per tile (128 or 256) for `count` problems of d's geometry. g_variant decides for every launch when it is
+// not 0; MTT_GEMM_GROUPED_VARIANT (0 auto, 1, 2) is an A/B knob for grouped launches (count > 1) only. Otherwise the
+// choice is made by tile counts, not per-shape timings.
+static int tile_width(const mtt_gemm_desc* d, int count) {
+  static int grouped = -1;
+  if (g_variant < 0) {
+    const char* e = getenv("MTT_GEMM_VARIANT");
+    g_variant = e ? atoi(e) : 0;
+  }
+  if (grouped < 0) {
+    const char* e = getenv("MTT_GEMM_GROUPED_VARIANT");
+    grouped = e ? atoi(e) : 0;
+  }
+  int v = g_variant;
+  if (v == 0 && count > 1) v = grouped;
+  if (v == 0) {
+    const int n256 = (d->N + 255) / 256 * 256;
+    const long long wide_tiles = (long long)count * ((d->M + 127) / 128) * (n256 / 256);
+    if (count > 1) {
+      // Grouping can fill the SMs with 128 x 256 tiles where one problem alone could not: with >= one wave of wide
+      // tiles and N close to a multiple of 256 they take the wide kernel. Gathered-A problems and tiny M stay on
+      // 128 x 128.
+      v = (d->a_group_rows == 0 && d->M >= 512 && d->N >= 256 && (n256 - d->N) * 8 <= n256 && wide_tiles >= sm_count())
+              ? 2 : 1;
+    } else if (d->mode == 1) {
+      // The 128 x 256 tile reads half the B bytes per output of the 128 x 128 tile and gives each consumer warpgroup a
+      // 64 x 256 wgmma; it needs enough tiles to fill the SMs and little waste in the last N tile. Narrow or ragged N
+      // (decoder widths 300 / 350), short K and skinny M stay on 128 x 128.
+      const long long k_eff = (long long)d->K * d->ksize * d->ksize;
+      v = (k_eff >= 2048 && wide_tiles >= sm_count() && d->N > 256 && (n256 - d->N) * 8 <= n256) ? 2 : 1;
+    } else {
+      const bool wide = d->N >= 512 && (n256 - d->N) * 8 <= n256;
+      v = (wide && d->M > 128 && (d->N >= 2048 || d->K >= 2048)) ? 2 : 1;
+    }
+  }
+  return v == 2 ? 256 : 128;
+}
 
 }  // namespace mtt
 
@@ -195,29 +223,11 @@ extern "C" size_t mtt_gemm_streamk_bytes(void) {
 extern "C" int mtt_gemm(const mtt_gemm_desc* d, mtt_stream_t stream_) {
   using namespace mtt;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (g_variant < 0) {
-    const char* e = getenv("MTT_GEMM_VARIANT");
-    g_variant = e ? atoi(e) : 0;
-  }
-  int v = g_variant;
-  if (v == 0) {
-    // The 128 x 256 tile reads half the B bytes per output of the 128 x 128 tile and gives each consumer warpgroup a
-    // 64 x 256 wgmma; it needs enough tiles to fill the SMs and little waste in the last N tile. Narrow or ragged N
-    // (decoder widths 300 / 350), short K and skinny M stay on 128 x 128. Chosen by tile counts, not per-shape timings.
-    if (!d) return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm: null descriptor");
-    const int n256 = (d->N + 255) / 256 * 256;
-    const long long wide_tiles = (long long)((d->M + 127) / 128) * (n256 / 256);
-    if (d->mode == 1) {
-      const long long k_eff = (long long)d->K * d->ksize * d->ksize;
-      v = (k_eff >= 2048 && wide_tiles >= sm_count() && d->N > 256 && (n256 - d->N) * 8 <= n256) ? 2 : 1;
-    } else {
-      const bool wide = d->N >= 512 && (n256 - d->N) * 8 <= n256;
-      v = (wide && d->M > 128 && (d->N >= 2048 || d->K >= 2048)) ? 2 : 1;
-    }
-  }
-  const int taps = (d && d->mode == 1) ? d->ksize * d->ksize : 1;
-  ProfileScope prof(stream, 0, d ? 2.0 * d->M * d->N * d->K * taps : 0.0, d ? d->M : 0, d ? d->N : 0, d ? d->K * taps : 0);
-  return launch_gemm_tiles(d, v == 2 ? 256 : 128, stream);
+  if (!d) return set_error(MTT_ERR_BAD_SHAPE, "mtt_gemm: null descriptor");
+  const int bn = tile_width(d, 1);
+  const int taps = d->mode == 1 ? d->ksize * d->ksize : 1;
+  ProfileScope prof(stream, 0, 2.0 * d->M * d->N * d->K * taps, d->M, d->N, d->K * taps);
+  return launch_gemm_tiles(d, bn, stream);
 }
 
 extern "C" int mtt_gemm_grouped(const mtt_gemm_desc* d, int32_t count, mtt_stream_t stream_) {
@@ -243,23 +253,5 @@ extern "C" int mtt_gemm_grouped(const mtt_gemm_desc* d, int32_t count, mtt_strea
   double fl = 0;
   for (int g = 0; g < count; ++g) fl += 2.0 * d[g].M * d[g].N * d[g].K * (d[g].mode == 1 ? d[g].ksize * d[g].ksize : 1);
   ProfileScope prof(stream, 0, fl, a.M * count, a.N, a.K * (a.mode == 1 ? a.ksize * a.ksize : 1));
-  if (g_variant < 0) {
-    const char* e = getenv("MTT_GEMM_VARIANT");
-    g_variant = e ? atoi(e) : 0;
-  }
-  int v = g_variant;
-  static int g_grouped = -1;  // MTT_GEMM_GROUPED_VARIANT: A/B knob for grouped launches only (0 auto, 1, 2)
-  if (g_grouped < 0) {
-    const char* e = getenv("MTT_GEMM_GROUPED_VARIANT");
-    g_grouped = e ? atoi(e) : 0;
-  }
-  if (v == 0) v = g_grouped;
-  if (v == 0) {
-    // Grouping can fill the SMs with 128 x 256 tiles where one problem alone could not: with >= one wave of wide tiles
-    // and N close to a multiple of 256 they take the wide kernel. Gathered-A problems and tiny M stay on 128 x 128.
-    const int n256 = (a.N + 255) / 256 * 256;
-    const long long wide_tiles = (long long)count * ((a.M + 127) / 128) * (n256 / 256);
-    v = (a.a_group_rows == 0 && a.M >= 512 && a.N >= 256 && (n256 - a.N) * 8 <= n256 && wide_tiles >= sm_count()) ? 2 : 1;
-  }
-  return launch_gemm_tiles_grouped(d, count, v == 2 ? 256 : 128, stream);
+  return launch_gemm_tiles_grouped(d, count, tile_width(d, count), stream);
 }
