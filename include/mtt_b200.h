@@ -305,6 +305,16 @@ typedef struct {
 size_t mtt_augment_workspace_bytes(int32_t B);
 int mtt_augment(const mtt_augment_desc* d, mtt_stream_t stream);
 
+/* Cityscapes-3D targets (TP/data/cityscapes3d.py:150-160 disparity, :235-241 encode_segmap, :206-228 PIL NEAREST
+ * resize to dd_label_map_size) over a batch of equally sized raw maps, in one launch. label_ids: uint8 [B,h,w] (the
+ * gtFine labelIds PNGs); disparity: uint16 [B,h,w] (the disparity PNGs), needed when depth is requested. Outputs at
+ * H x W (H x W == h x w: no resize): semseg int64 [B,H,W] -- void ids -> 255, the 19 valid ids -> 0..18, other ids
+ * unchanged; depth fp32 [B,1,H,W] -- (d - 1) / 256 for d > 1, -1 for d <= 1 (the reference's in-place steps also turn
+ * d == 1 into -1), 0 where the raw label id is 10 (as the reference masks it). Either output may be NULL, not both. Source pixels follow Pillow's NEAREST rule, restated in
+ * oracle/cityscapes_ref.py. */
+int mtt_cityscapes_targets(const uint8_t* label_ids, const uint16_t* disparity, int32_t B, int32_t h, int32_t w,
+                           int32_t H, int32_t W, int64_t* semseg, float* depth, mtt_stream_t stream);
+
 /* Predictions -> uint8 images, for the reference's prediction export (save_model_pred_for_one_task,
  * TP/evaluation/evaluate_utils.py:69-151, IP/evaluation/evaluate_utils.py:69-105) and inference visualisation
  * (vis_pred_for_one_task, TP/utils/visualization_utils.py:80-199). One descriptor per task; all (task, image) pairs of
@@ -557,6 +567,9 @@ size_t mtt_meter_state_bytes(int32_t kind, int32_t n);
 int mtt_meter_reset(void* state, int32_t kind, int32_t n, mtt_stream_t stream);
 int mtt_meter_confusion_update(const int64_t* pred, const float* label, int32_t B, int32_t H, int32_t W,
                                int32_t n_classes, float ignore_index, void* state, mtt_stream_t stream);
+/* The same update with int64 labels [B,H,W] (the Cityscapes-3D loader's semseg, TP/data/cityscapes3d.py:227). */
+int mtt_meter_confusion_update_i64(const int64_t* pred, const int64_t* label, int32_t B, int32_t H, int32_t W,
+                                   int32_t n_classes, float ignore_index, void* state, mtt_stream_t stream);
 int mtt_meter_saliency_update(const float* pred, const float* label, int32_t B, int32_t H, int32_t W,
                               const float* thresholds, int32_t n_thresholds, float ignore_index, void* state,
                               mtt_stream_t stream);

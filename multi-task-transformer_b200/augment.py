@@ -88,11 +88,15 @@ _IDENTITY = dict(scale=1.0, crops=None, flip=False, bright=None, f_mode=False, c
 
 
 def _collate_meta(metas):
-    """collate_mil (TP/utils/custom_collate.py) on the datasets' meta dicts: names as a list, sizes as LongTensors."""
+    """collate_mil (TP/utils/custom_collate.py) on the datasets' meta dicts: names as a list, sizes as LongTensors,
+    numpy arrays stacked (Cityscapes-3D's scale_factor)."""
     out = {}
     for k in metas[0]:
         vals = [m[k] for m in metas]
-        out[k] = [torch.LongTensor(list(v)) for v in vals] if isinstance(vals[0], (tuple, list)) else vals
+        if isinstance(vals[0], np.ndarray):
+            out[k] = torch.stack([torch.from_numpy(v) for v in vals], 0)
+        else:
+            out[k] = [torch.LongTensor(list(v)) for v in vals] if isinstance(vals[0], (tuple, list)) else vals
     return out
 
 

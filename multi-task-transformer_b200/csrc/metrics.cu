@@ -78,18 +78,26 @@ __device__ void fixed_order_add(const double (&v)[NS], double* __restrict__ sums
 }
 
 // ---- confusion counts (SemsegMeter eval_semseg.py:70-81, HumanPartsMeter eval_human_parts.py:33-42) -----------------
+// The label's gt bin: a class 0..n-1 or n ("any other value"); fp32 maps (the transforms' [B,1,H,W]) and int64 maps
+// (the Cityscapes-3D loader's [B,H,W]) compare with ignore the way torch compares them with the Python number.
+__device__ __forceinline__ bool label_ignored(float g, float ignore) { return g == ignore; }
+__device__ __forceinline__ bool label_ignored(long long g, float ignore) { return (double)g == (double)ignore; }
+__device__ __forceinline__ int label_bin(float g, int n) { return (g >= 0.f && g < (float)n && g == floorf(g)) ? (int)g : n; }
+__device__ __forceinline__ int label_bin(long long g, int n) { return (g >= 0 && g < n) ? (int)g : n; }
+
+template <typename Label>
 __global__ void __launch_bounds__(kMeterThreads)
-confusion_kernel(const long long* __restrict__ pred, const float* __restrict__ label, long long npix, int n,
+confusion_kernel(const long long* __restrict__ pred, const Label* __restrict__ label, long long npix, int n,
                  float ignore, unsigned long long* __restrict__ M) {
   extern __shared__ unsigned int hist[];
   const int nb = n + 1, bins = nb * nb;
   for (int i = threadIdx.x; i < bins; i += blockDim.x) hist[i] = 0u;
   __syncthreads();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (long long)gridDim.x * blockDim.x) {
-    const float g = label[i];
-    if (g == ignore) continue;
+    const Label g = label[i];
+    if (label_ignored(g, ignore)) continue;
     const long long p = pred[i];
-    const int gb = (g >= 0.f && g < (float)n && g == floorf(g)) ? (int)g : n;
+    const int gb = label_bin(g, n);
     const int pb = (p >= 0 && p < n) ? (int)p : n;
     atomicAdd(&hist[gb * nb + pb], 1u);
   }
@@ -287,18 +295,37 @@ int mtt_meter_reset(void* state, int32_t kind, int32_t n, mtt_stream_t stream) {
   return MTT_OK;
 }
 
-int mtt_meter_confusion_update(const int64_t* pred, const float* label, int32_t B, int32_t H, int32_t W,
-                               int32_t n_classes, float ignore_index, void* state, mtt_stream_t stream) {
-  int rc = meter_args("mtt_meter_confusion_update", pred, label, state, B, H, W);
+}  // extern "C"
+
+namespace mtt {
+
+template <typename Label>
+int confusion_update(const char* what, const int64_t* pred, const Label* label, int32_t B, int32_t H, int32_t W,
+                     int32_t n_classes, float ignore_index, void* state, mtt_stream_t stream) {
+  int rc = meter_args(what, pred, label, state, B, H, W);
   if (rc) return rc;
   if (n_classes < 1 || n_classes > kMeterMaxClasses)
-    return set_error(MTT_ERR_BAD_SHAPE, "mtt_meter_confusion_update: %d classes (histogram capacity %d)", n_classes,
-                     kMeterMaxClasses);
+    return set_error(MTT_ERR_BAD_SHAPE, "%s: %d classes (histogram capacity %d)", what, n_classes, kMeterMaxClasses);
   const long long npix = (long long)B * H * W;
   const size_t smem = (size_t)(n_classes + 1) * (n_classes + 1) * sizeof(unsigned int);
-  confusion_kernel<<<meter_blocks(npix, 16), kMeterThreads, smem, STREAM>>>(
+  confusion_kernel<Label><<<meter_blocks(npix, 16), kMeterThreads, smem, STREAM>>>(
       reinterpret_cast<const long long*>(pred), label, npix, n_classes, ignore_index, STATE);
-  return check_launch("mtt_meter_confusion_update");
+  return check_launch(what);
+}
+
+}  // namespace mtt
+
+extern "C" {
+
+int mtt_meter_confusion_update(const int64_t* pred, const float* label, int32_t B, int32_t H, int32_t W,
+                               int32_t n_classes, float ignore_index, void* state, mtt_stream_t stream) {
+  return confusion_update("mtt_meter_confusion_update", pred, label, B, H, W, n_classes, ignore_index, state, stream);
+}
+
+int mtt_meter_confusion_update_i64(const int64_t* pred, const int64_t* label, int32_t B, int32_t H, int32_t W,
+                                   int32_t n_classes, float ignore_index, void* state, mtt_stream_t stream) {
+  return confusion_update("mtt_meter_confusion_update_i64", pred, reinterpret_cast<const long long*>(label), B, H, W,
+                          n_classes, ignore_index, state, stream);
 }
 
 int mtt_meter_saliency_update(const float* pred, const float* label, int32_t B, int32_t H, int32_t W,

@@ -145,6 +145,7 @@ SYMBOLS = {
     "mtt_bilinear_postproc": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "mtt_augment_workspace_bytes": (C.c_size_t, [_i32]),
     "mtt_augment": (C.c_int, [C.POINTER(AugmentDesc), _vp]),
+    "mtt_cityscapes_targets": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "mtt_render_workspace_bytes": (C.c_size_t, [_i32, _i32]),
     "mtt_render": (C.c_int, [C.POINTER(RenderDesc), _i32, _vp, _vp]),
     "mtt_render_jet_bgr": (C.POINTER(C.c_uint8), []),
@@ -182,6 +183,7 @@ SYMBOLS = {
     "mtt_meter_state_bytes": (C.c_size_t, [_i32, _i32]),
     "mtt_meter_reset": (C.c_int, [_vp, _i32, _i32, _vp]),
     "mtt_meter_confusion_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
+    "mtt_meter_confusion_update_i64": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp]),
     "mtt_meter_saliency_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _i32, _f32, _vp, _vp]),
     "mtt_meter_normals_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _f32, _vp, _vp]),
     "mtt_meter_depth_update": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _f32, _f32, _f32, _vp, _vp]),

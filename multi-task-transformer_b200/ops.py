@@ -332,12 +332,18 @@ def meter_reset(state, kind, n=0):
     _L.check(_L.load().mtt_meter_reset(_ptr(state), int(kind), int(n), _stream()), "mtt_meter_reset")
 
 
-def _meter_inputs(what, pred, pred_dtype, pred_shape, label, label_channels, state):
+def _meter_inputs(what, pred, pred_dtype, pred_shape, label, label_channels, state, int64_labels=False):
     """Validates a meter update's tensors before any launch: dtypes, shapes (pred_shape(B, H, W) from the label's
-    [B, label_channels, H, W]), contiguity and device. Returns (B, H, W)."""
-    if label.dtype != torch.float32 or label.dim() != 4 or label.shape[1] != label_channels:
-        raise ValueError(f"{what}: label must be fp32 [B,{label_channels},H,W], got {label.dtype} {tuple(label.shape)}")
-    B, _, H, W = (int(s) for s in label.shape)
+    [B, label_channels, H, W], or int64 [B, H, W] where int64_labels allows it), contiguity and device.
+    Returns (B, H, W)."""
+    if int64_labels and label.dtype == torch.int64 and label.dim() == 3:
+        B, H, W = (int(s) for s in label.shape)
+    elif label.dtype != torch.float32 or label.dim() != 4 or label.shape[1] != label_channels:
+        also = " or int64 [B,H,W]" if int64_labels else ""
+        raise ValueError(f"{what}: label must be fp32 [B,{label_channels},H,W]{also}, got {label.dtype} "
+                         f"{tuple(label.shape)}")
+    else:
+        B, _, H, W = (int(s) for s in label.shape)
     if pred.dtype != pred_dtype or tuple(pred.shape) != pred_shape(B, H, W):
         raise ValueError(f"{what}: prediction must be {pred_dtype} {pred_shape(B, H, W)} for a label of shape "
                          f"{tuple(label.shape)}, got {pred.dtype} {tuple(pred.shape)}")
@@ -349,11 +355,14 @@ def _meter_inputs(what, pred, pred_dtype, pred_shape, label, label_channels, sta
 
 
 def meter_confusion_update(pred, label, n_classes, ignore_index, state):
-    """pred int64 [B,H,W] class map, label fp32 [B,1,H,W]."""
-    B, H, W = _meter_inputs("meter_confusion_update", pred, torch.int64, lambda b, h, w: (b, h, w), label, 1, state)
-    rc = _L.load().mtt_meter_confusion_update(_ptr(pred), _ptr(label), B, H, W, int(n_classes), float(ignore_index),
-                                              _ptr(state), _stream())
-    _L.check(rc, "mtt_meter_confusion_update")
+    """pred int64 [B,H,W] class map, label fp32 [B,1,H,W] (the transforms' format) or int64 [B,H,W] (the Cityscapes-3D
+    loader's, TP/data/cityscapes3d.py:227); the reference meter squeezes both the same way (eval_semseg.py:71-81)."""
+    B, H, W = _meter_inputs("meter_confusion_update", pred, torch.int64, lambda b, h, w: (b, h, w), label, 1, state,
+                            int64_labels=True)
+    fn = "mtt_meter_confusion_update_i64" if label.dtype == torch.int64 else "mtt_meter_confusion_update"
+    rc = getattr(_L.load(), fn)(_ptr(pred), _ptr(label), B, H, W, int(n_classes), float(ignore_index), _ptr(state),
+                                _stream())
+    _L.check(rc, fn)
 
 
 def meter_saliency_update(pred, label, thresholds, ignore_index, state):
@@ -416,6 +425,31 @@ def preprocess_image(img_u8, out_hw, *, bgr=True, mean=IMAGENET_MEAN, std=IMAGEN
     rc = _L.load().mtt_preprocess_image(_ptr(img_u8), B, h, w, int(bool(bgr)), m3, s3, _ptr(out), H, W, _stream())
     _L.check(rc, "mtt_preprocess_image")
     return out
+
+
+def cityscapes_targets(label_ids, disparity, out_hw, *, semseg=None, depth=None):
+    """The reference's Cityscapes-3D targets (mtt_cityscapes_targets): label_ids uint8 [B,h,w] and disparity uint16
+    [B,h,w] (or None when no depth is asked for) on the device -> semseg int64 [B,H,W] and / or depth fp32 [B,1,H,W]
+    at out_hw = (H, W), written into the given tensors."""
+    if label_ids.dtype != torch.uint8 or label_ids.dim() != 3 or not label_ids.is_cuda:
+        raise ValueError(f"cityscapes_targets: label ids must be CUDA uint8 [B,h,w], got {label_ids.dtype} "
+                         f"{tuple(label_ids.shape)} on {label_ids.device}")
+    B, h, w = (int(s) for s in label_ids.shape)
+    H, W = (int(s) for s in out_hw)
+    if semseg is None and depth is None:
+        raise ValueError("cityscapes_targets: no output requested")
+    if depth is not None and (disparity is None or disparity.dtype != torch.uint16 or
+                              tuple(disparity.shape) != (B, h, w) or not disparity.is_cuda):
+        raise ValueError(f"cityscapes_targets: depth needs a CUDA uint16 disparity of shape {(B, h, w)}")
+    for name, t, dt, shape in (("semseg", semseg, torch.int64, (B, H, W)), ("depth", depth, torch.float32, (B, 1, H, W))):
+        if t is not None and (t.dtype != dt or tuple(t.shape) != shape or not t.is_cuda):
+            raise ValueError(f"cityscapes_targets: {name} must be CUDA {dt} {shape}, got {t.dtype} {tuple(t.shape)}")
+    for t in (label_ids, disparity, semseg, depth):
+        if t is not None and not t.is_contiguous():
+            raise ValueError("cityscapes_targets: every tensor must be contiguous")
+    rc = _L.load().mtt_cityscapes_targets(_ptr(label_ids), _ptr(disparity if depth is not None else None), B, h, w, H,
+                                          W, _ptr(semseg), _ptr(depth), _stream())
+    _L.check(rc, "mtt_cityscapes_targets")
 
 
 def augment_workspace_bytes(B):

@@ -39,7 +39,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .plans import Plan, _cached, _dev_ctx, _f32, _lin, _pack_stem
+from .plans import Plan, _cached, _dev_ctx, _f32, _lin, _pack_stem, _predict_outputs
 from .taskprompter import (PARITY, Mlp, PatchEmbed, _HeadSpace, _launch_head, _pack_fuse, _pack_head,
                            _trunc_normal_)
 
@@ -265,14 +265,17 @@ def _pack_swin_decoder(bb, tasks, device, ns):
 # the fused forward
 # --------------------------------------------------------------------------------------------
 class _SwinPlan(Plan):
-    """Geometry, workspace and launch sequence of one TaskPrompterSwin wrapper forward."""
+    """Geometry, workspace and launch sequence of one TaskPrompterSwin wrapper forward. mode: "full" = wrapper forward
+    (logits at the output size), "postproc" = predict() (get_output fused into the final resize, same launch count)."""
 
     def __init__(self, bb, heads, tasks, target, B, device, nsplit, mode="full"):
         super().__init__((bb, heads), B, device, nsplit, max(len(tasks), 2))
-        if mode not in ("full",):
-            raise NotImplementedError("mtt_b200 TaskPrompterSwin: only the wrapper forward is built (no predict())")
+        if mode not in ("full", "postproc"):
+            raise NotImplementedError(f"mtt_b200 TaskPrompterSwin: no {mode!r} plan (the wrapper forward and predict() "
+                                      "are built)")
         device = self.dev
         self.bb, self.heads, self.tasks, self.target, self.mode = bb, heads, list(tasks), target, mode
+        self.postproc = mode == "postproc"
         self.T = T = len(self.tasks)
         p = bb.p
         self.ce = ce = p.chan_embed_dim
@@ -361,7 +364,10 @@ class _SwinPlan(Plan):
             self.hs = [_HeadSpace(hw, B, h0, w0, device, ns) for hw in self.Wh]
             oh, ow = self.target if self.target is not None else self.img
             self.out_hw = (oh, ow)
-            self.out = {t: z(B, hw.n_out, oh, ow) for t, hw in zip(self.tasks, self.Wh)}
+            if self.postproc:
+                self.out = _predict_outputs(self.tasks, B, (oh, ow), device)
+            else:
+                self.out = {t: z(B, hw.n_out, oh, ow) for t, hw in zip(self.tasks, self.Wh)}
 
     def _pack(self):
         bb, dev, ns = self.bb, self.dev, self.ns
@@ -448,7 +454,11 @@ class _SwinPlan(Plan):
         ops.split_f32(self.acc[ti][:, :self.f], self.ns, out=self.accs[ti])
         ops.gemm(self.accs[ti], wm, N=self.f, K=self.f, bias=bm, out_split=hs.up, conv=(B, self.fh, self.fw, 3, 1))  # :717
         _launch_head(hs, hw)
-        ops.bilinear(hs.pred, hs.pred.stride(0), B, hs.ph, hs.pw, hw.n_out, oh, ow, out_nchw=self.out[t])  # wrapper :35
+        if self.postproc:
+            ops.bilinear_postproc(hs.pred, hs.pred.stride(0), B, hs.ph, hs.pw, hw.n_out, oh, ow,
+                                  ops.POSTPROC_KIND[t], self.out[t])                         # wrapper :35 + utils.py:27-63
+        else:
+            ops.bilinear(hs.pred, hs.pred.stride(0), B, hs.ph, hs.pw, hw.n_out, oh, ow, out_nchw=self.out[t])  # :35
 
     def _launch(self, img):
         B, T, bb, W = self.B, self.T, self.bb, self.Ws
