@@ -264,6 +264,15 @@ def _pack_swin_decoder(bb, tasks, device, ns):
 # --------------------------------------------------------------------------------------------
 # the fused forward
 # --------------------------------------------------------------------------------------------
+def chan_kv_chunks(rows, ce, L):
+    """K chunks of chan_kv, Linear(H*W -> 2 ce) over `rows` = B*C rows: few output tiles, very long K. K is split so that
+    about one wave of 148 CTAs is busy (K chunks are multiples of 64, at least 512 columns each). 148 is the B200's SM
+    count (the H100 has 132); the chunk count sets the order of the fp32 summation, so a retune changes the results in
+    the last bits."""
+    tiles = -(-rows // 128) * -(-(2 * ce) // 128)
+    return max(1, min(32, 148 // tiles, L // 512))
+
+
 class _SwinPlan(Plan):
     """Geometry, workspace and launch sequence of one TaskPrompterSwin wrapper forward. mode: "full" = wrapper forward
     (logits at the output size), "postproc" = predict() (get_output fused into the final resize, same launch count)."""
@@ -322,10 +331,7 @@ class _SwinPlan(Plan):
                 s.q32 = z(B * T, ce)
                 s.xat = S(B * C, L, zero=True)
                 s.kv32 = z(B * C, 2 * ce)
-                # chan_kv is Linear(H*W -> 2 ce) over B*C rows: few output tiles, very long K. Split K so that about one
-                # wave of 148 CTAs is busy (K chunks are multiples of 64, at least 512 columns each)
-                tiles = -(-(B * C) // 128) * -(-(2 * ce) // 128)
-                s.kchunks = max(1, min(32, 148 // tiles, L // 512))
+                s.kchunks = chan_kv_chunks(B * C, ce, L)
                 s.kv_part = z(s.kchunks, B * C, 2 * ce) if s.kchunks > 1 else None
                 s.co32, s.cos = z(B * T, ce), S(B * T, ce)
                 s.t1 = S(B * T, ce)

@@ -187,13 +187,19 @@ def make_losses():
 # (ii) the exact norms of the full tensors, and (iii) for multi-class tasks the full-resolution arg-max map
 # (uint8) with the mask of pixels whose top-2 margin exceeds 1e-4 * max|logit| (where arg-max must be exact).
 # The input is regenerated from the seed; its SHA-256 is stored.
+# Fixtures listed in BIG_XZ are written xz-compressed (big_<cfg>_b<batch>.pt.xz) with a coarser lattice: the Swin-B model
+# has 19 output channels at 512 x 1024, whose stride-8 lattice alone is 620 KB of fp32 that does not compress; at stride
+# 16 (39 k points, about 9 per stage-1 attention window of the output) the file is about 140 KB, the full-resolution
+# arg-max map compressing to about 1 KB. The norm and the arg-max map still cover every pixel.
 BIG_STRIDE = 8
+BIG_XZ = {"tps_swinB": 16}     # config -> lattice stride
 BIG_JOBS = [  # (family, config, seed, batch)
     ("taskprompter", "tp_cfg5_d4", 41, 1),   # N = 8195 tokens: 65 query tiles, ragged last key block
     ("taskprompter", "tp_cfg4", 42, 4),      # the bench configuration: 24 blocks, bs 4
     ("taskprompter", "tp_cfg2", 43, 4),      # BASELINE.json configs[1]
     ("invpt", "ip_cfg3", 44, 4),             # BASELINE.json configs[2]
     ("taskprompter", "tp_cfg5", 45, 1),      # BASELINE.json configs[4]: full 24-block, N = 8195
+    ("taskprompter_swin", "tps_swinB", 46, 1),   # Swin-B Cityscapes-3D 1024x2048: ws 12, T 2, four stages
 ]
 
 
@@ -208,12 +214,12 @@ def lattice(b, ti, H, W, stride=BIG_STRIDE):
     return torch.arange(oy, H, stride), torch.arange(ox, W, stride)
 
 
-def compress_output(y, ti, with_argmax=True):
+def compress_output(y, ti, with_argmax=True, stride=BIG_STRIDE):
     """y [B, n_out, H, W] fp32 -> the fixture record described above (`safe` is bit-packed, numpy.packbits order)."""
     B, n, H, W = y.shape
     samp = []
     for b in range(B):
-        iy, ix = lattice(b, ti, H, W)
+        iy, ix = lattice(b, ti, H, W, stride)
         samp.append(y[b][:, iy][:, :, ix].clone())
     rec = {"shape": tuple(y.shape), "samples": torch.stack(samp), "norm": float(y.double().norm()),
            "absmax": float(y.abs().max())}
@@ -231,20 +237,30 @@ def make_big(family, name, seed, batch):
         from oracle import taskprompter_ref as R
         cfg = configs.taskprompter(name)
         model = ref_loader.build_taskprompter(cfg).eval()
+    elif family == "taskprompter_swin":
+        from oracle import taskprompter_swin_ref as R
+        cfg = configs.taskprompter_swin(name)
+        model = ref_loader.build_taskprompter_swin(cfg).eval()
     else:
         from oracle import invpt_ref as R
         cfg = configs.invpt(name)
         model = ref_loader.build_invpt(cfg).eval()
     sd = R.init_state_dict(cfg, seed=seed)
-    model.load_state_dict(sd, strict=True)
+    if family == "taskprompter_swin":
+        missing, unexpected = model.load_state_dict(sd, strict=False)   # index / mask buffers are derived, not stored
+        assert not unexpected and all("relative_position_index" in k or "attn_mask" in k for k in missing), (missing, unexpected)
+    else:
+        model.load_state_dict(sd, strict=True)
     x = big_input(cfg, seed, batch)
     with torch.no_grad():
         y = model(x)
-    out = {t: compress_output(y[t], ti) for ti, t in enumerate(cfg["tasks"])}
+    stride = BIG_XZ.get(name, BIG_STRIDE)
+    out = {t: compress_output(y[t], ti, stride=stride) for ti, t in enumerate(cfg["tasks"])}
     inter = None
     if family == "invpt":
-        inter = {t: compress_output(y["inter_preds"][t], ti, with_argmax=False) for ti, t in enumerate(cfg["tasks"])}
-    return {"family": family, "cfg": name, "seed": seed, "batch": batch, "stride": BIG_STRIDE, "out": out,
+        inter = {t: compress_output(y["inter_preds"][t], ti, with_argmax=False, stride=stride)
+                 for ti, t in enumerate(cfg["tasks"])}
+    return {"family": family, "cfg": name, "seed": seed, "batch": batch, "stride": stride, "out": out,
             "inter_preds": inter, "x_sha256": hashlib.sha256(x.numpy().tobytes()).hexdigest(),
             "sd_sha256": sd_checksum(sd), "torch": torch.__version__,
             "made_by": "oracle/make_golden.py make_big: unmodified reference forward (eval, fp32, CPU), lattice-sampled"}
@@ -258,7 +274,13 @@ def main_big(only=None):
         t0 = time.time()
         fx = make_big(fam, name, seed, batch)
         path = os.path.join(GOLD, f"big_{name}_b{batch}.pt")
-        torch.save(fx, path)
+        if name in BIG_XZ:
+            import lzma
+            path += ".xz"
+            with lzma.open(path, "wb", preset=9 | lzma.PRESET_EXTREME) as f:
+                torch.save(fx, f)
+        else:
+            torch.save(fx, path)
         print(f"wrote {path} ({os.path.getsize(path) / 1024:.0f} KiB, {time.time() - t0:.0f} s)", flush=True)
 
 

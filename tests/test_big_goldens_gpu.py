@@ -7,6 +7,8 @@ CUDA-graph replay the bench uses, against golden vectors made here by the UNMODI
   big_tp_cfg4_b4      the bench configuration: ViT-L PASCAL 512x512, 24 blocks, bs 4, graph replay
   big_tp_cfg2_b4      ViT-B NYUD 448x576 bs 4 (configs[1])
   big_ip_cfg3_b4      InvPT ViT-L PASCAL 512x512 bs 4 (configs[2])
+  big_tps_swinB_b1    Swin-B TaskPrompter Cityscapes-3D 1024x2048 bs 1, stride-16 lattice, .pt.xz (tests/test_swin_big_gpu.py:
+                      forward and predict())
 
 A fixture holds every output value on a stride-8 pixel lattice (offset varies per image and task), the exact
 norm and max of the full tensors, and for multi-class tasks the full-resolution arg-max map plus the mask of
