@@ -664,9 +664,10 @@ int mtt_nhwc_to_nchw(const float* in, int64_t ld_in, int32_t B, int32_t C, int32
  * mtt_transpose_planes: bf16 planes [B][R][C] (image b at row b*in_batch_rows) -> image b's [C, R] block at element offset
  *   b*out_batch_stride of the output (0 = C*ld_out: blocks stacked by rows; R: side by side along the columns); exact.
  * mtt_bn_stats / mtt_bn_finalize / mtt_bn_act: train-mode BatchNorm2d over NHWC rows: sums = (sum x, sum x^2) per channel
- *   [2*cols] (all-reduce them across ranks for SyncBatchNorm, main.py:92), mean_rstd [2*cols] from sums / count with the
- *   running statistics updated like nn.BatchNorm2d (momentum, unbiased running_var), then y = act(xhat*gamma + beta) as
- *   fp32 and / or split planes. mtt_bn_bwd_reduce: sums = (sum dz, sum dz*xhat), dz = dy * act'(z) (= dbeta, dgamma; all-reduce
+ *   [2*cols] accumulated in DOUBLE (all-reduce them across ranks for SyncBatchNorm, main.py:92), mean_rstd [2*cols] from
+ *   sums / count with the variance sum x^2 / count - mean^2 formed in double (in fp32 that subtraction loses ~1e-6
+ *   (mean/std)^2 of the variance, in double ~1e-16 (mean/std)^2) and the running statistics updated like nn.BatchNorm2d
+ *   (momentum, unbiased running_var), then y = act(xhat*gamma + beta) as fp32 and / or split planes. mtt_bn_bwd_reduce: sums = (sum dz, sum dz*xhat), dz = dy * act'(z) (= dbeta, dgamma; all-reduce
  *   for SyncBatchNorm); mtt_bn_bwd_apply: dx = gamma*rstd*(dz - sums[0]/count - xhat*sums[1]/count).
  * mtt_attn_softmax_bwd: per (batch*head) rows of raw scores S [BH, N, ld] and dP [BH, N, ld] (fp32, read only):
  *   P = softmax(scale*S) recomputed, dS = scale*P*(dP - delta) with delta [BH, N] = sum_j P dP = rowdot(dO, O) from
@@ -686,7 +687,8 @@ int mtt_nhwc_to_nchw(const float* in, int64_t ld_in, int32_t B, int32_t C, int32
  *   rows (c, ky, kx) in nn.Conv2d.weight order, columns = output pixels (ldo >= B*H*W).
  * mtt_sumsq + mtt_adam_step: clip_grad_norm_(max_norm, 2) and torch.optim.Adam on flat fp32 arenas (p, g, m, v of n
  *   elements): g is scaled by grad_scale (1 / world size after a sum all-reduce) and by min(1, max_norm / (norm + 1e-6))
- *   when gnorm_sq (device scalar, sum of squared gradients BEFORE grad_scale) is given; weight decay is Adam's L2 form. */
+ *   when gnorm_sq (device scalar, sum of squared gradients BEFORE grad_scale) is given; weight decay is Adam's L2 form.
+ *   beta1 / beta2 are double (as torch.optim.Adam keeps them): 1 - beta and the bias corrections are formed from them. */
 int mtt_colsum(const float* x, int64_t ldx, int64_t rows, int32_t cols, int64_t in_group, int64_t src_group, int64_t src_offset,
                float* out, int32_t accumulate, mtt_stream_t stream);
 int mtt_layernorm_bwd(const float* x, int64_t ldx, const float* dy, int64_t lddy, const float* gamma, float eps, int64_t rows,
@@ -701,8 +703,8 @@ int mtt_axpy_rows(const float* base, int64_t ldb, const float* src, int64_t lds,
 int mtt_transpose_planes(const void* in_hi, const void* in_lo, int64_t ld_in, int64_t in_batch_rows, int32_t B, int32_t R,
                          int32_t C, void* out_hi, void* out_lo, int64_t ld_out, int64_t out_batch_stride,
                          mtt_stream_t stream);
-int mtt_bn_stats(const float* x, int64_t ldx, int64_t rows, int32_t cols, float* sums, mtt_stream_t stream);
-int mtt_bn_finalize(const float* sums, float count, int32_t cols, float eps, float momentum, float* mean_rstd,
+int mtt_bn_stats(const float* x, int64_t ldx, int64_t rows, int32_t cols, double* sums, mtt_stream_t stream);
+int mtt_bn_finalize(const double* sums, double count, int32_t cols, float eps, float momentum, float* mean_rstd,
                     float* running_mean, float* running_var, mtt_stream_t stream);
 int mtt_bn_act(const float* x, int64_t ldx, int64_t rows, int32_t cols, const float* mean_rstd, const float* gamma,
                const float* beta, int32_t act, float* out_f32, int64_t ldo, void* out_hi, void* out_lo, int64_t ldbf,
@@ -736,7 +738,7 @@ int mtt_im2col3x3_t(const float* x, int64_t ldx, int32_t B, int32_t H, int32_t W
 int mtt_im2col_patch_t(const float* img, int32_t B, int32_t Cin, int32_t H, int32_t W, int32_t patch, void* out_hi,
                        void* out_lo, int64_t ldo, mtt_stream_t stream);
 int mtt_sumsq(const float* g, int64_t n, float* out, int32_t accumulate, mtt_stream_t stream);
-int mtt_adam_step(float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2, float eps,
+int mtt_adam_step(float* p, const float* g, float* m, float* v, int64_t n, float lr, double beta1, double beta2, float eps,
                   float weight_decay, int32_t step, const float* gnorm_sq, float max_norm, float grad_scale,
                   mtt_stream_t stream);
 

@@ -31,6 +31,9 @@ def taskprompter(name):
         # a 2-block slice of cfg4 geometry for full-size kernel parity at low cost
         "tp_cfg4_d4": dict(tasks=PASCAL_TASKS, num_output=PASCAL_OUT, img_size=(512, 512), patch=16, C=1024,
                            depth=4, heads=16, select=[1, 2, 3], e=300, f=350, chan_nheads=1, use_ctr=True),
+        # a 4-block slice of cfg2 geometry (4 x 4 channel windows, e = f = 768, no ctr) for the reverse pass at full width
+        "tp_cfg2_d4": dict(tasks=NYUD_TASKS, num_output=NYUD_OUT, img_size=(448, 576), patch=16, C=768, depth=4,
+                           heads=12, select=[1, 2, 3], e=768, f=768, chan_nheads=16, use_ctr=False),
         # BASELINE.json configs[4] stand-in (SURVEY.md section 0 row 5)
         "tp_cfg5": dict(tasks=["semseg", "depth", "3ddet"], num_output={"semseg": 19, "depth": 1, "3ddet": 18},
                         img_size=(1024, 2048), patch=16, C=1024, depth=24, heads=16, select=[6, 12, 18],

@@ -39,7 +39,8 @@ __device__ __forceinline__ float act_grad(float z, int act) {
 
 // ---- column reductions ----------------------------------------------------------------------------------------------
 // out1[c] += sum_r v1(r, c), out2[c] += sum_r v2(r, c): block = 32 columns x 8 row lanes, grid.y row chunks, one atomicAdd
-// per (block, column). The caller zeroes the outputs unless it accumulates.
+// per (block, column); sums in Acc (float, or double for the BatchNorm statistics). The caller zeroes the outputs unless it
+// accumulates.
 struct SumOp {          // bias gradients: v1 = x; logical row r = (g, i), i < in_group, at row g*src_group + src_offset + i
   const float* x; long long ld; long long in_group, src_group, src_offset;
   __device__ void operator()(long long r, int c, float& a, float& b) const {
@@ -48,9 +49,12 @@ struct SumOp {          // bias gradients: v1 = x; logical row r = (g, i), i < i
     b = 0.f;
   }
 };
-struct StatsOp {        // BatchNorm batch statistics: v1 = x, v2 = x^2
+struct StatsOp {        // BatchNorm batch statistics in double: v1 = x, v2 = x^2 (exact: a float's square fits a double)
   const float* x; long long ld;
-  __device__ void operator()(long long r, int c, float& a, float& b) const { a = x[r * ld + c]; b = a * a; }
+  __device__ void operator()(long long r, int c, double& a, double& b) const {
+    a = (double)x[r * ld + c];
+    b = a * a;
+  }
 };
 struct BnBwdOp {        // v1 = dz, v2 = dz * xhat with dz = dy * act'(z), z = xhat * gamma + beta
   const float* x; long long ldx; const float* dy; long long lddy;
@@ -70,16 +74,16 @@ struct LnBwdOp {        // v1 = dy (dbeta), v2 = dy * xhat (dgamma); per-row sta
   }
 };
 
-template <class Op>
+template <class Op, class Acc>
 __global__ void __launch_bounds__(256)
-colreduce_kernel(Op op, long long rows, int cols, float* __restrict__ out1, float* __restrict__ out2) {
-  __shared__ float s1[8][33], s2[8][33];
+colreduce_kernel(Op op, long long rows, int cols, Acc* __restrict__ out1, Acc* __restrict__ out2) {
+  __shared__ Acc s1[8][33], s2[8][33];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int c = blockIdx.x * 32 + tx;
-  float a1 = 0.f, a2 = 0.f;
+  Acc a1 = 0, a2 = 0;
   if (c < cols) {
     for (long long r = (long long)blockIdx.y * 8 + ty; r < rows; r += (long long)gridDim.y * 8) {
-      float u, v;
+      Acc u, v;
       op(r, c, u, v);
       a1 += u;
       a2 += v;
@@ -99,14 +103,14 @@ colreduce_kernel(Op op, long long rows, int cols, float* __restrict__ out1, floa
   }
 }
 
-template <class Op>
-int launch_colreduce(Op op, long long rows, int cols, float* out1, float* out2, cudaStream_t st, const char* what) {
+template <class Op, class Acc>
+int launch_colreduce(Op op, long long rows, int cols, Acc* out1, Acc* out2, cudaStream_t st, const char* what) {
   const int cb = (cols + 31) / 32;
   long long rb = (rows + 63) / 64;                       // >= 8 rows per row lane
   const long long cap = (long long)sm_count() * 8 / cb + 1;
   if (rb > cap) rb = cap;
   if (rb < 1) rb = 1;
-  colreduce_kernel<Op><<<dim3(cb, (unsigned)rb), 256, 0, st>>>(op, rows, cols, out1, out2);
+  colreduce_kernel<Op, Acc><<<dim3(cb, (unsigned)rb), 256, 0, st>>>(op, rows, cols, out1, out2);
   return check_launch(what);
 }
 
@@ -238,20 +242,22 @@ transpose_planes_kernel(const __nv_bfloat16* __restrict__ in_hi, const __nv_bflo
 }
 
 // ---- train-mode BatchNorm ----------------------------------------------------------------------------------------------
-__global__ void bn_finalize_kernel(const float* __restrict__ sums, float count, int cols, float eps, float momentum,
+// The variance is sum x^2 / n - mean^2 formed in double: the cancellation costs ~1e-16 (mean/std)^2 of it, where the same
+// subtraction over fp32 sums lost ~1e-6 (mean/std)^2 (1e-3 of the variance at mean/std = 30).
+__global__ void bn_finalize_kernel(const double* __restrict__ sums, double count, int cols, float eps, float momentum,
                                    float* __restrict__ mean_rstd, float* __restrict__ running_mean,
                                    float* __restrict__ running_var) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= cols) return;
-  const float mean = sums[c] / count;
-  float var = sums[cols + c] / count - mean * mean;      // biased (normalisation)
-  if (var < 0.f) var = 0.f;
-  mean_rstd[c] = mean;
-  mean_rstd[cols + c] = 1.0f / sqrtf(var + eps);
+  const double mean = sums[c] / count;
+  double var = sums[cols + c] / count - mean * mean;     // biased (normalisation)
+  if (var < 0.0) var = 0.0;
+  mean_rstd[c] = (float)mean;
+  mean_rstd[cols + c] = (float)(1.0 / sqrt(var + (double)eps));
   if (running_mean) {                                     // nn.BatchNorm2d: running_var takes the UNBIASED estimate
-    const float unb = count > 1.f ? var * count / (count - 1.f) : var;
-    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean;
-    running_var[c] = (1.f - momentum) * running_var[c] + momentum * unb;
+    const double unb = count > 1.0 ? var * count / (count - 1.0) : var;
+    running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)mean;
+    running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unb;
   }
 }
 
@@ -737,8 +743,8 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g,
 // clamped to 1): p, g, m, v flat fp32 arenas; gnorm_sq = sum of squared gradients (device scalar) or NULL = no clipping.
 __global__ void __launch_bounds__(256)
 adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long n,
-            float lr, float beta1, float beta2, float eps, float wd, float bc1, float bc2, const float* __restrict__ gnorm_sq,
-            float max_norm, float grad_scale) {
+            float lr, float beta1, float beta2, float omb1, float omb2, float eps, float wd, float bc1, float bc2,
+            const float* __restrict__ gnorm_sq, float max_norm, float grad_scale) {
   float clip = grad_scale;
   if (gnorm_sq) {
     const float nrm = sqrtf(*gnorm_sq) * grad_scale;
@@ -747,8 +753,8 @@ adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restric
   }
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const float gi = g[i] * clip + wd * p[i];
-    const float mi = beta1 * m[i] + (1.f - beta1) * gi;
-    const float vi = beta2 * v[i] + (1.f - beta2) * gi * gi;
+    const float mi = beta1 * m[i] + omb1 * gi;
+    const float vi = beta2 * v[i] + omb2 * gi * gi;
     m[i] = mi;
     v[i] = vi;
     p[i] -= lr / bc1 * mi / (sqrtf(vi) / sqrtf(bc2) + eps);
@@ -768,7 +774,8 @@ extern "C" int mtt_colsum(const float* x, int64_t ldx, int64_t rows, int32_t col
                           int64_t src_offset, float* out, int32_t accumulate, mtt_stream_t stream) {
   if (!x || !out || rows <= 0 || cols <= 0) return set_error(MTT_ERR_BAD_SHAPE, "mtt_colsum: bad arguments");
   if (!accumulate) cudaMemsetAsync(out, 0, sizeof(float) * cols, ST);
-  return launch_colreduce(SumOp{x, ldx, in_group, src_group, src_offset}, rows, cols, out, nullptr, ST, "mtt_colsum");
+  return launch_colreduce(SumOp{x, ldx, in_group, src_group, src_offset}, rows, cols, out, (float*)nullptr, ST,
+                          "mtt_colsum");
 }
 
 extern "C" int mtt_layernorm_bwd(const float* x, int64_t ldx, const float* dy, int64_t lddy, const float* gamma, float eps,
@@ -820,15 +827,15 @@ extern "C" int mtt_transpose_planes(const void* in_hi, const void* in_lo, int64_
   return check_launch("mtt_transpose_planes");
 }
 
-extern "C" int mtt_bn_stats(const float* x, int64_t ldx, int64_t rows, int32_t cols, float* sums, mtt_stream_t stream) {
+extern "C" int mtt_bn_stats(const float* x, int64_t ldx, int64_t rows, int32_t cols, double* sums, mtt_stream_t stream) {
   if (!x || !sums || rows <= 0 || cols <= 0) return set_error(MTT_ERR_BAD_SHAPE, "mtt_bn_stats: bad arguments");
-  cudaMemsetAsync(sums, 0, sizeof(float) * 2 * cols, ST);
+  cudaMemsetAsync(sums, 0, sizeof(double) * 2 * cols, ST);
   return launch_colreduce(StatsOp{x, ldx}, rows, cols, sums, sums + cols, ST, "mtt_bn_stats");
 }
 
-extern "C" int mtt_bn_finalize(const float* sums, float count, int32_t cols, float eps, float momentum, float* mean_rstd,
-                               float* running_mean, float* running_var, mtt_stream_t stream) {
-  if (!sums || !mean_rstd || cols <= 0 || count <= 0.f) return set_error(MTT_ERR_BAD_SHAPE, "mtt_bn_finalize: bad arguments");
+extern "C" int mtt_bn_finalize(const double* sums, double count, int32_t cols, float eps, float momentum,
+                               float* mean_rstd, float* running_mean, float* running_var, mtt_stream_t stream) {
+  if (!sums || !mean_rstd || cols <= 0 || count <= 0.0) return set_error(MTT_ERR_BAD_SHAPE, "mtt_bn_finalize: bad arguments");
   bn_finalize_kernel<<<(cols + 127) / 128, 128, 0, ST>>>(sums, count, cols, eps, momentum, mean_rstd, running_mean,
                                                          running_var);
   return check_launch("mtt_bn_finalize");
@@ -975,15 +982,18 @@ extern "C" int mtt_sumsq(const float* g, int64_t n, float* out, int32_t accumula
   return check_launch("mtt_sumsq");
 }
 
-extern "C" int mtt_adam_step(float* p, const float* g, float* m, float* v, int64_t n, float lr, float beta1, float beta2,
+extern "C" int mtt_adam_step(float* p, const float* g, float* m, float* v, int64_t n, float lr, double beta1, double beta2,
                              float eps, float weight_decay, int32_t step, const float* gnorm_sq, float max_norm,
                              float grad_scale, mtt_stream_t stream) {
   if (!p || !g || !m || !v || n <= 0 || step <= 0) return set_error(MTT_ERR_BAD_SHAPE, "mtt_adam_step: bad arguments");
   long long blocks = (n + 255) / 256;
   const long long cap = (long long)sm_count() * 8;
   if (blocks > cap) blocks = cap;
-  const float bc1 = 1.f - powf(beta1, (float)step), bc2 = 1.f - powf(beta2, (float)step);
-  adam_kernel<<<(unsigned)blocks, 256, 0, ST>>>(p, g, m, v, n, lr, beta1, beta2, eps, weight_decay, bc1, bc2, gnorm_sq,
-                                                max_norm, grad_scale);
+  // 1 - beta and the bias corrections from the double betas: 1 - (float)0.999 is 1.3e-5 off 0.001, and so is
+  // 1 - 0.999f^step, which would scale v's increment and the step by that much against torch.optim.Adam
+  const float bc1 = (float)(1.0 - pow(beta1, (double)step)), bc2 = (float)(1.0 - pow(beta2, (double)step));
+  adam_kernel<<<(unsigned)blocks, 256, 0, ST>>>(p, g, m, v, n, lr, (float)beta1, (float)beta2, (float)(1.0 - beta1),
+                                                (float)(1.0 - beta2), eps, weight_decay, bc1, bc2, gnorm_sq, max_norm,
+                                                grad_scale);
   return check_launch("mtt_adam_step");
 }

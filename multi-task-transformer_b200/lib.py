@@ -212,7 +212,7 @@ SYMBOLS = {
     "mtt_axpy_rows": (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _vp, _i64, _vp]),
     "mtt_transpose_planes": (C.c_int, [_vp, _vp, _i64, _i64, _i32, _i32, _i32, _vp, _vp, _i64, _i64, _vp]),
     "mtt_bn_stats": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _vp]),
-    "mtt_bn_finalize": (C.c_int, [_vp, _f32, _i32, _f32, _f32, _vp, _vp, _vp, _vp]),
+    "mtt_bn_finalize": (C.c_int, [_vp, C.c_double, _i32, _f32, _f32, _vp, _vp, _vp, _vp]),
     "mtt_bn_act": (C.c_int, [_vp, _i64, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _i64, _vp, _vp, _i64, _vp]),
     "mtt_bn_bwd_reduce": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _vp]),
     "mtt_bn_bwd_apply": (C.c_int, [_vp, _i64, _vp, _i64, _i64, _i32, _vp, _vp, _vp, _i32, _vp, _f32, _vp, _i64, _vp]),
@@ -228,7 +228,8 @@ SYMBOLS = {
     "mtt_im2col3x3_t": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
     "mtt_im2col_patch_t": (C.c_int, [_vp, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
     "mtt_sumsq": (C.c_int, [_vp, _i64, _vp, _i32, _vp]),
-    "mtt_adam_step": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _f32, _f32, _f32, _i32, _vp, _f32, _f32, _vp]),
+    "mtt_adam_step": (C.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, C.c_double, C.c_double, _f32, _f32, _i32, _vp, _f32, _f32,
+                                _vp]),
 }
 
 _lib = None

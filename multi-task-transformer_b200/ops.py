@@ -898,11 +898,18 @@ def transpose_planes(a, *, B=1, R=None, Ccols=None, in_batch_rows=None, out=None
 
 
 def bn_stats(x, sums):
-    _L.check(_L.load().mtt_bn_stats(_ptr(x), _ld(x), x.shape[0], x.shape[1], _ptr(sums), _stream()), "mtt_bn_stats")
+    """sums [2C] = (sum x, sum x^2) over the rows of x, accumulated in float64. Keep sums float64 (TrainStep does): a
+    float32 buffer receives the rounded sums, and the variance formed from those cancels in fp32 as |mean| / std grows."""
+    out = sums if sums.dtype == torch.float64 else torch.empty(sums.shape, dtype=torch.float64, device=sums.device)
+    _L.check(_L.load().mtt_bn_stats(_ptr(x), _ld(x), x.shape[0], x.shape[1], _ptr(out), _stream()), "mtt_bn_stats")
+    if out is not sums:
+        sums.copy_(out)
 
 
 def bn_finalize(sums, count, eps, momentum, mean_rstd, running_mean=None, running_var=None):
-    _L.check(_L.load().mtt_bn_finalize(_ptr(sums), float(count), sums.numel() // 2, float(eps), float(momentum),
+    """mean_rstd [2C] fp32 from sums (float64, or float32 widened) / count, the variance formed in float64."""
+    s = sums if sums.dtype == torch.float64 else sums.double()
+    _L.check(_L.load().mtt_bn_finalize(_ptr(s), float(count), s.numel() // 2, float(eps), float(momentum),
                                        _ptr(mean_rstd), _ptr(running_mean), _ptr(running_var), _stream()), "mtt_bn_finalize")
 
 

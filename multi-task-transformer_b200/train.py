@@ -254,9 +254,11 @@ class TrainStep:
         return out
 
     def _bn_fwd(self, x, prefix, act, out_split):
-        """Train-mode BatchNorm2d `prefix` (+ act) over NHWC rows x -> out_split; returns the saved statistics."""
+        """Train-mode BatchNorm2d `prefix` (+ act) over NHWC rows x -> out_split; returns the saved statistics. The sums
+        (sum x, sum x^2) are float64, all-reduced as such with a process group (SyncBatchNorm), so the variance
+        sum x^2 / n - mean^2 does not cancel in fp32 when a channel's |mean| >> std."""
         C_ = x.shape[1]
-        sums = _e(2 * C_, device=self.dev)
+        sums = torch.empty(2 * C_, dtype=torch.float64, device=self.dev)
         ops.bn_stats(x, sums)
         count = x.shape[0]
         if self.pg is not None:
