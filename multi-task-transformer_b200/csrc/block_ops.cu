@@ -8,8 +8,8 @@
 //   mtt_ln_mlp_residual   :274,:277 (norm2, Mlp fc1 + GELU + fc2, residual)                LayerNorm -> GEMM+GELU -> GEMM+residual
 //   mtt_gated_conv1x1     :436-447, :452-468, :471 (spatial + channel gating, two 1x1)     gate kernel -> 2 GEMMs into the cat buffer
 //   mtt_conv3x3_bn_act    :362 / :691-695 (3x3 + BN + act, optional fused 1x1 head)        implicit-GEMM conv (-> GEMM)
+#include "glue.cuh"
 #include "host_common.h"
-#include "ptx.cuh"
 
 namespace mtt {
 
@@ -32,11 +32,7 @@ pack_conv_kernel(const float* __restrict__ w, const float* __restrict__ scale, i
       v = transposed ? w[((long long)c * N + n) * taps + (taps - 1 - tap)] : w[((long long)n * Cin + c) * taps + tap];
       if (scale) v *= scale[n];
     }
-    __nv_bfloat16 h, l;
-    split_bf16(v, h, l);
-    const long long o = (long long)n * ld + (long long)tap * cin_pad + c;
-    hi[o] = h;
-    if (lo) lo[o] = l;
+    store_split({hi, lo, ld}, n, (long long)tap * cin_pad + c, v);
   }
 }
 
@@ -72,11 +68,7 @@ nchw_to_nhwc_split_kernel(const float* __restrict__ in, int C, int HW, __nv_bflo
   __syncthreads();
   const int p = p0 + ty, c = c0 + tx;
   if (p < HW && c < C) {
-    __nv_bfloat16 h, l;
-    split_bf16(tile[tx][ty], h, l);
-    const long long o = ((long long)b * HW + p) * ld + c;
-    hi[o] = h;
-    if (lo) lo[o] = l;
+    store_split({hi, lo, ld}, (long long)b * HW + p, c, tile[tx][ty]);
   }
 }
 

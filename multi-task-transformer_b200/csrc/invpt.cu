@@ -5,27 +5,10 @@
 // cross-task attention with cross-scale score fusion.
 #include <math.h>
 
+#include "glue.cuh"
 #include "host_common.h"
-#include "ptx.cuh"
 
 namespace mtt {
-
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float warp_max_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-// physical row of logical row r: (r / in_group) * src_group + src_off + r % in_group
-__device__ __forceinline__ long long map_row(long long r, long long in_group, long long src_group,
-                                             long long src_off) {
-  return in_group > 0 ? (r / in_group) * src_group + src_off + r % in_group : r + src_off;
-}
 
 // ------------------------------------------------------------------------------------------------
 // fp32 rows (gathered) -> split planes (dense).  e.g. x[:, 1:] of the ViT stream (vit.py:345-346).
@@ -39,19 +22,7 @@ split_rows_kernel(const float* __restrict__ in, long long ld_in, long long in_gr
   const float* src = in + map_row(row, in_group, src_group, src_off) * ld_in;
   for (int c = lane * 2; c < cols; c += 64) {
     const bool two = c + 1 < cols;
-    uint32_t h, l;
-    split_pack2(src[c], two ? src[c + 1] : 0.f, h, l);
-    if (two && !(ld_out & 1)) {
-      *reinterpret_cast<uint32_t*>(hi + row * ld_out + c) = h;
-      if (lo) *reinterpret_cast<uint32_t*>(lo + row * ld_out + c) = l;
-    } else {
-      hi[row * ld_out + c] = __ushort_as_bfloat16((unsigned short)(h & 0xFFFF));
-      if (lo) lo[row * ld_out + c] = __ushort_as_bfloat16((unsigned short)(l & 0xFFFF));
-      if (two) {
-        hi[row * ld_out + c + 1] = __ushort_as_bfloat16((unsigned short)(h >> 16));
-        if (lo) lo[row * ld_out + c + 1] = __ushort_as_bfloat16((unsigned short)(l >> 16));
-      }
-    }
+    store_split2({hi, lo, ld_out}, row, c, src[c], two ? src[c + 1] : 0.f, two && !(ld_out & 1), two);
   }
 }
 
@@ -77,7 +48,7 @@ layernorm_seg_kernel(const float* __restrict__ in, long long ld_in, long long in
     const float* src = base + (long long)k * seg_stride * ld_in;
     for (int c = lane; c < cols; c += 32) s += src[c];
   }
-  const float mean = warp_sum_f(s) / n;
+  const float mean = warp_sum(s) / n;
   float ss = 0.f;
   for (int k = 0; k < S; ++k) {
     const float* src = base + (long long)k * seg_stride * ld_in;
@@ -86,19 +57,14 @@ layernorm_seg_kernel(const float* __restrict__ in, long long ld_in, long long in
       ss += a * a;
     }
   }
-  const float rstd = 1.0f / sqrtf(warp_sum_f(ss) / n + eps);
+  const float rstd = 1.0f / sqrtf(warp_sum(ss) / n + eps);
   for (int k = 0; k < S; ++k) {
     const float* src = base + (long long)k * seg_stride * ld_in;
     const long long orow = (long long)k * out_seg_stride + row;
     for (int c = lane; c < cols; c += 32) {
       const float y = (src[c] - mean) * rstd * gamma[k * cols + c] + beta[k * cols + c];
       if (out_f32) out_f32[orow * ld_f32 + c] = y;
-      if (out_hi) {
-        __nv_bfloat16 h, l;
-        split_bf16(y, h, l);
-        out_hi[orow * ld_bf + c] = h;
-        if (out_lo) out_lo[orow * ld_bf + c] = l;
-      }
+      if (out_hi) store_split({out_hi, out_lo, ld_bf}, orow, c, y);
     }
   }
 }
@@ -150,10 +116,7 @@ dwconv_s2_kernel(const float* __restrict__ in, long long ld_in, int T, int h, in
         acc = fmaf(wc[ky * 3 + kx], base[((long long)iy * w + ix) * ld_in + c], acc);
       }
     }
-    __nv_bfloat16 hh, ll;
-    split_bf16(acc, hh, ll);
-    hi[orow * ld_out + c] = hh;
-    if (lo) lo[orow * ld_out + c] = ll;
+    store_split({hi, lo, ld_out}, orow, c, acc);
   }
 }
 
@@ -172,10 +135,7 @@ avgpool_kernel(const float* __restrict__ in, long long ld_in, int h, int w, int 
     float acc = 0.f;
     for (int y = y0; y < y1; ++y)
       for (int x = x0; x < x1; ++x) acc += base[((long long)y * w + x) * ld_in + c];
-    __nv_bfloat16 hh, ll;
-    split_bf16(acc * inv, hh, ll);
-    hi[orow * ld_out + c] = hh;
-    if (lo) lo[orow * ld_out + c] = ll;
+    store_split({hi, lo, ld_out}, orow, c, acc * inv);
   }
 }
 
@@ -251,8 +211,8 @@ invpt_fuse_softmax_kernel(const float* __restrict__ raw, int B, int Lq, int Tk, 
       m1 = fmaxf(m1, s1);
     }
   }
-  m0 = warp_max_f(m0);
-  m1 = warp_max_f(m1);
+  m0 = warp_max(m0);
+  m1 = warp_max(m1);
   float z0 = 0.f, z1 = 0.f;
 #pragma unroll
   for (int k = 0; k < kFuseMaxPerLane; ++k) {
@@ -263,7 +223,7 @@ invpt_fuse_softmax_kernel(const float* __restrict__ raw, int B, int Lq, int Tk, 
       z1 += f1[k];
     }
   }
-  const float i0 = 1.0f / warp_sum_f(z0), i1 = 1.0f / warp_sum_f(z1);
+  const float i0 = 1.0f / warp_sum(z0), i1 = 1.0f / warp_sum(z1);
   __nv_bfloat16* h0 = p_hi + (((long long)b * 2 + 0) * Lq + l) * ldp;
   __nv_bfloat16* h1 = p_hi + (((long long)b * 2 + 1) * Lq + l) * ldp;
 #pragma unroll

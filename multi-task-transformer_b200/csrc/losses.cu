@@ -11,6 +11,7 @@
 // the same state. state layout (double[8]): 0 n_valid, 1 n_neg (sum of 1 - y over valid), 2 loss sum, 3 loss value.
 #include <math.h>
 
+#include "glue.cuh"
 #include "host_common.h"
 #include "loss_terms.cuh"
 
@@ -18,19 +19,6 @@ namespace mtt {
 
 constexpr int kLossThreads = 256;
 constexpr int kLossMaxBlocks = 1024;
-
-__device__ __forceinline__ double block_sum(double v, double* sh) {
-  // fixed-order tree over the block: deterministic
-  sh[threadIdx.x] = v;
-  __syncthreads();
-  for (int s = blockDim.x >> 1; s > 0; s >>= 1) {
-    if (threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
-    __syncthreads();
-  }
-  const double r = sh[0];
-  __syncthreads();
-  return r;
-}
 
 // ---- (1) label statistics: n_valid and sum(1 - y) over valid entries; `all_channels`: a pixel is valid when every
 // channel of the label differs from ignore (L1Loss :163), counted once per pixel.

@@ -16,6 +16,7 @@
 // result is bitwise reproducible for a given shape, and the ticket is back at 0 when the launch ends.
 #include <math.h>
 
+#include "glue.cuh"
 #include "host_common.h"
 #include "loss_terms.cuh"
 
@@ -29,30 +30,6 @@ constexpr int kMeterMaxSums = 4;
 
 // float kinds: [header words][ticket][kMeterMaxBlocks * nsums partial doubles]
 constexpr int kNormalsHeader = 2, kDepthHeader = 5, kEdgeHeader = 2;
-
-__device__ __forceinline__ double block_sum_d(double v, double* sh) {
-  sh[threadIdx.x] = v;
-  __syncthreads();
-  for (int s = blockDim.x >> 1; s > 0; s >>= 1) {
-    if (threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
-    __syncthreads();
-  }
-  const double r = sh[0];
-  __syncthreads();
-  return r;
-}
-
-__device__ __forceinline__ unsigned long long block_sum_u(unsigned long long v, unsigned long long* sh) {
-  sh[threadIdx.x] = v;
-  __syncthreads();
-  for (int s = blockDim.x >> 1; s > 0; s >>= 1) {
-    if (threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
-    __syncthreads();
-  }
-  const unsigned long long r = sh[0];
-  __syncthreads();
-  return r;
-}
 
 // Adds this CTA's NS fp64 sums to sums[0..NS) in a fixed order: every CTA parks its values in its slots; the last CTA
 // to arrive adds the slots of blocks 0, 1, 2, ... in turn and resets the ticket.
@@ -139,15 +116,15 @@ saliency_kernel(const float* __restrict__ pred, const float* __restrict__ label,
 #pragma unroll
   for (int k = 0; k < kMeterMaxThresholds; ++k) {
     if (k < T) {   // T is uniform: every thread takes the same branches through the block sums
-      const unsigned long long a = block_sum_u((unsigned long long)tp[k], sh);
-      const unsigned long long b = block_sum_u((unsigned long long)pp[k], sh);
+      const unsigned long long a = block_sum((unsigned long long)tp[k], sh);
+      const unsigned long long b = block_sum((unsigned long long)pp[k], sh);
       if (threadIdx.x == 0) {
         atomicAdd(&tp_g[k], a);
         atomicAdd(&pp_g[k], b);
       }
     }
   }
-  const unsigned long long a = block_sum_u((unsigned long long)ap, sh);
+  const unsigned long long a = block_sum((unsigned long long)ap, sh);
   if (threadIdx.x == 0)
     for (int k = 0; k < T; ++k) atomicAdd(&ap_g[k], a);
 }
@@ -184,8 +161,8 @@ normals_kernel(const float* __restrict__ pred_nhwc, const float* __restrict__ la
     acc += (double)(rad * (float)(180.0 / M_PI));
     cnt += 1;
   }
-  const double v[1] = {block_sum_d(acc, sh)};
-  cnt = block_sum_u(cnt, shu);
+  const double v[1] = {block_sum(acc, sh)};
+  cnt = block_sum(cnt, shu);
   if (threadIdx.x == 0) atomicAdd(&st[1], cnt);
   fixed_order_add<1>(v, reinterpret_cast<double*>(st), reinterpret_cast<unsigned int*>(st + kNormalsHeader),
                      reinterpret_cast<double*>(st + kNormalsHeader + 1));
@@ -213,8 +190,8 @@ depth_kernel(const float* __restrict__ pred, const float* __restrict__ label, lo
     s3 += (double)(d * d / g);
     cnt += 1;
   }
-  const double v[4] = {block_sum_d(s0, sh), block_sum_d(s1, sh), block_sum_d(s2, sh), block_sum_d(s3, sh)};
-  cnt = block_sum_u(cnt, shu);
+  const double v[4] = {block_sum(s0, sh), block_sum(s1, sh), block_sum(s2, sh), block_sum(s3, sh)};
+  cnt = block_sum(cnt, shu);
   if (threadIdx.x == 0) atomicAdd(&st[0], cnt);
   fixed_order_add<4>(v, reinterpret_cast<double*>(st + 1), reinterpret_cast<unsigned int*>(st + kDepthHeader),
                      reinterpret_cast<double*>(st + kDepthHeader + 1));
@@ -235,8 +212,8 @@ edge_kernel(const float* __restrict__ pred, const float* __restrict__ label, lon
     acc += (double)balanced_bce_term(pred[i] / 255.f, y, pos_weight);
     cnt += 1;
   }
-  const double v[1] = {block_sum_d(acc, sh)};
-  cnt = block_sum_u(cnt, shu);
+  const double v[1] = {block_sum(acc, sh)};
+  cnt = block_sum(cnt, shu);
   if (threadIdx.x == 0) atomicAdd(&st[1], cnt);
   fixed_order_add<1>(v, reinterpret_cast<double*>(st), reinterpret_cast<unsigned int*>(st + kEdgeHeader),
                      reinterpret_cast<double*>(st + kEdgeHeader + 1));

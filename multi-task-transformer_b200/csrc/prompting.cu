@@ -5,9 +5,9 @@
 // waves of 132 SMs at the benchmark shapes).
 #include <stdlib.h>
 
+#include "glue.cuh"
 #include "host_common.h"
 #include "postproc.cuh"
-#include "ptx.cuh"
 
 namespace mtt {
 
@@ -26,10 +26,7 @@ im2col_patch_kernel(const float* __restrict__ img, int Cin, int H, int W, int pa
     const int r = k % (patch * patch);
     const int ky = r / patch, kx = r % patch;
     const float v = img[(((long long)b * Cin + c) * H + py * patch + ky) * W + px * patch + kx];
-    __nv_bfloat16 h, l;
-    split_bf16(v, h, l);
-    hi[row * ld + k] = h;
-    if (lo) lo[row * ld + k] = l;
+    store_split({hi, lo, ld}, row, k, v);
   }
 }
 
@@ -112,9 +109,8 @@ gate_split_kernel(const float* __restrict__ x, long long ldx, long long x_group,
   const int P = gh * gw;
   const long long row = blockIdx.x;  // b * P + pix
   const int b = (int)(row / P), pix = (int)(row % P);
-  const int py = pix / gw, px = pix % gw;
   const int nwin = nh * nw;
-  const int win = (py / (gh / nh)) * nw + px / (gw / nw);
+  const int win = chan_window(pix, gh, gw, nh, nw);
   const float* xr = x + ((long long)b * x_group + x_off + pix) * ldx;
   for (int c = threadIdx.x * 8; c < C; c += blockDim.x * 8) {
     const float4 xa = *reinterpret_cast<const float4*>(xr + c), xb = *reinterpret_cast<const float4*>(xr + c + 4);

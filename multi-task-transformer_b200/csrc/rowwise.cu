@@ -1,15 +1,9 @@
 // Row-wise HBM-bound kernels: fp32 -> split-bf16 cast and LayerNorm with split output.
 // One warp per row, float4 loads, warp-shuffle reductions.
+#include "glue.cuh"
 #include "host_common.h"
-#include "ptx.cuh"
 
 namespace mtt {
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 
 __global__ void __launch_bounds__(256)
 split_kernel(const float* __restrict__ in, long long ld_in, __nv_bfloat16* __restrict__ hi,

@@ -8,8 +8,8 @@
 // row-major order (TP:177-181 puts the prompts FIRST in every window).
 #include <math.h>
 
+#include "glue.cuh"
 #include "host_common.h"
-#include "ptx.cuh"
 
 namespace mtt {
 
@@ -223,16 +223,8 @@ transpose_split_kernel(const float* __restrict__ in, long long ld_in, int L, int
     const int c = c0 + warp * 4 + k;
     const int l = l0 + 2 * lane;
     if (c >= C || l >= L) continue;
-    uint32_t hh, ll;
-    split_pack2(tile[2 * lane][warp * 4 + k], tile[2 * lane + 1][warp * 4 + k], hh, ll);
-    const long long o = ((long long)b * C + c) * ld + l;
-    if (l + 1 < L) {
-      *reinterpret_cast<uint32_t*>(hi + o) = hh;
-      if (lo) *reinterpret_cast<uint32_t*>(lo + o) = ll;
-    } else {
-      hi[o] = __ushort_as_bfloat16((unsigned short)(hh & 0xFFFF));
-      if (lo) lo[o] = __ushort_as_bfloat16((unsigned short)(ll & 0xFFFF));
-    }
+    store_split2({hi, lo, ld}, (long long)b * C + c, l, tile[2 * lane][warp * 4 + k], tile[2 * lane + 1][warp * 4 + k],
+                 l + 1 < L, false);
   }
 }
 
@@ -263,8 +255,7 @@ swin_chan_attn_kernel(const float* __restrict__ q, long long ldq, const float* _
     const float* kr = kv + ((long long)b * C + c) * ldkv;
     float s = 0.f;
     for (int e = lane; e < we; e += 32) s = fmaf(sq[e], kr[eidx(e)], s);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    s = warp_sum(s);
     if (lane == 0) {
       if (blockIdx.y == 0) rc[(((long long)b * T + t) * C + c) * (nh * nw) + g] = s;   // raw_chan [B,T,C,nh,nw] (TP:391)
       sp[c] = s * scale;
@@ -312,10 +303,7 @@ swin_chan_attn_kernel(const float* __restrict__ q, long long ldq, const float* _
     tot *= inv;
     const long long orow = (long long)b * T + t;
     co[orow * ldco + col] = tot;
-    __nv_bfloat16 h, l;
-    split_bf16(tot, h, l);
-    cs_hi[orow * ldcs + col] = h;
-    if (cs_lo) cs_lo[orow * ldcs + col] = l;
+    store_split({cs_hi, cs_lo, ldcs}, orow, col, tot);
   }
 }
 

@@ -3,23 +3,13 @@
 // gradients), row-wise LayerNorm and softmax backward, the train-mode BatchNorm (batch statistics), the adjoints of the
 // bilinear resize and of the spatial / channel gating, plane transposes that turn the K-major wgmma GEMM (mtt_gemm)
 // into its dgrad / wgrad forms, and the fused Adam + clip step. Contractions stay on mtt_gemm / mtt_gemm_grouped.
+#include "glue.cuh"
 #include "host_common.h"
-#include "ptx.cuh"
+#include "postproc.cuh"
 
 namespace mtt {
 
 namespace {
-
-__device__ __forceinline__ float wsum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ float wmax(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
 
 __device__ __forceinline__ float act_fwd(float z, int act) {
   if (act == MTT_ACT_GELU) return gelu_erf(z);
@@ -44,7 +34,7 @@ __device__ __forceinline__ float act_grad(float z, int act) {
 struct SumOp {          // bias gradients: v1 = x; logical row r = (g, i), i < in_group, at row g*src_group + src_offset + i
   const float* x; long long ld; long long in_group, src_group, src_offset;
   __device__ void operator()(long long r, int c, float& a, float& b) const {
-    const long long pr = in_group > 0 ? (r / in_group) * src_group + src_offset + r % in_group : r;
+    const long long pr = in_group > 0 ? map_row(r, in_group, src_group, src_offset) : r;   // no groups: src_offset unused
     a = x[pr * ld + c];
     b = 0.f;
   }
@@ -126,21 +116,21 @@ ln_bwd_rows_kernel(const float* __restrict__ x, long long ldx, const float* __re
   const float* gr = dy + row * lddy;
   float s = 0.f;
   for (int c = lane; c < cols; c += 32) s += xr[c];
-  const float mean = wsum(s) / (float)cols;
+  const float mean = warp_sum(s) / (float)cols;
   float ss = 0.f;
   for (int c = lane; c < cols; c += 32) {
     const float a = xr[c] - mean;
     ss += a * a;
   }
-  const float rstd = 1.0f / sqrtf(wsum(ss) / (float)cols + eps);
+  const float rstd = 1.0f / sqrtf(warp_sum(ss) / (float)cols + eps);
   float m1 = 0.f, m2 = 0.f;
   for (int c = lane; c < cols; c += 32) {
     const float g = gr[c] * gamma[c];
     m1 += g;
     m2 += g * (xr[c] - mean) * rstd;
   }
-  m1 = wsum(m1) / (float)cols;
-  m2 = wsum(m2) / (float)cols;
+  m1 = warp_sum(m1) / (float)cols;
+  m2 = warp_sum(m2) / (float)cols;
   float* o = dx + row * lddx;
   for (int c = lane; c < cols; c += 32) {
     const float xh = (xr[c] - mean) * rstd;
@@ -161,12 +151,7 @@ act_split_kernel(const float* __restrict__ pre, long long ld, long long rows, in
   const long long row = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
   if (row >= rows) return;
   const int lane = threadIdx.x & 31;
-  for (int c = lane; c < cols; c += 32) {
-    __nv_bfloat16 h, l;
-    split_bf16(act_fwd(pre[row * ld + c], act), h, l);
-    hi[row * ldo + c] = h;
-    if (lo) lo[row * ldo + c] = l;
-  }
+  for (int c = lane; c < cols; c += 32) store_split({hi, lo, ldo}, row, c, act_fwd(pre[row * ld + c], act));
 }
 
 __global__ void __launch_bounds__(256)
@@ -272,12 +257,7 @@ bn_act_kernel(const float* __restrict__ x, long long ldx, long long rows, int co
     const float xh = (x[row * ldx + c] - mean_rstd[c]) * mean_rstd[cols + c];
     const float y = act_fwd(xh * gamma[c] + beta[c], act);
     if (out_f32) out_f32[row * ldo + c] = y;
-    if (hi) {
-      __nv_bfloat16 h, l;
-      split_bf16(y, h, l);
-      hi[row * ldbf + c] = h;
-      if (lo) lo[row * ldbf + c] = l;
-    }
+    if (hi) store_split({hi, lo, ldbf}, row, c, y);
   }
 }
 
@@ -333,8 +313,8 @@ attn_softmax_bwd_kernel(const float* __restrict__ S, const float* __restrict__ d
         l += __expf(v - m);
       }
     }
-    const float mw = wmax(m);
-    l = wsum(l * __expf(m - mw));
+    const float mw = warp_max(m);
+    l = warp_sum(l * __expf(m - mw));
     if (lane == 0) {
       stat[warp * 8 + k][0] = mw;
       stat[warp * 8 + k][1] = 1.f / l;
@@ -366,16 +346,7 @@ attn_softmax_bwd_kernel(const float* __restrict__ S, const float* __restrict__ d
           d0 += dr[0];
           if (two) d1 += dr[1];
         }
-        uint32_t hh, ll;
-        split_pack2(d0, d1, hh, ll);
-        const long long o = (bh * N + q) * ldbf + kk;
-        if (two) {
-          *reinterpret_cast<uint32_t*>(ds_hi + o) = hh;
-          if (ds_lo) *reinterpret_cast<uint32_t*>(ds_lo + o) = ll;
-        } else {
-          ds_hi[o] = __ushort_as_bfloat16((unsigned short)(hh & 0xFFFF));
-          if (ds_lo) ds_lo[o] = __ushort_as_bfloat16((unsigned short)(ll & 0xFFFF));
-        }
+        store_split2({ds_hi, ds_lo, ldbf}, bh * N + q, kk, d0, d1, two, false);
       }
       tp[ql][2 * lane] = p0;
       tp[ql][2 * lane + 1] = p1;
@@ -390,24 +361,8 @@ attn_softmax_bwd_kernel(const float* __restrict__ S, const float* __restrict__ d
         const int q = q0 + 2 * lane;
         if (key >= N || q >= N) continue;
         const bool two = q + 1 < N;
-        const long long o = (bh * N + key) * ldbf + q;
-        uint32_t hh, ll;
-        split_pack2(tp[2 * lane][kl], tp[2 * lane + 1][kl], hh, ll);
-        if (two) {
-          *reinterpret_cast<uint32_t*>(pt_hi + o) = hh;
-          if (pt_lo) *reinterpret_cast<uint32_t*>(pt_lo + o) = ll;
-        } else {
-          pt_hi[o] = __ushort_as_bfloat16((unsigned short)(hh & 0xFFFF));
-          if (pt_lo) pt_lo[o] = __ushort_as_bfloat16((unsigned short)(ll & 0xFFFF));
-        }
-        split_pack2(td[2 * lane][kl], td[2 * lane + 1][kl], hh, ll);
-        if (two) {
-          *reinterpret_cast<uint32_t*>(dst_hi + o) = hh;
-          if (dst_lo) *reinterpret_cast<uint32_t*>(dst_lo + o) = ll;
-        } else {
-          dst_hi[o] = __ushort_as_bfloat16((unsigned short)(hh & 0xFFFF));
-          if (dst_lo) dst_lo[o] = __ushort_as_bfloat16((unsigned short)(ll & 0xFFFF));
-        }
+        store_split2({pt_hi, pt_lo, ldbf}, bh * N + key, q, tp[2 * lane][kl], tp[2 * lane + 1][kl], two, false);
+        store_split2({dst_hi, dst_lo, ldbf}, bh * N + key, q, td[2 * lane][kl], td[2 * lane + 1][kl], two, false);
       }
     }
     __syncthreads();
@@ -431,21 +386,12 @@ attn_delta_kernel(const float* __restrict__ dO, long long lddo, const __nv_bfloa
       if (o_lo) o += __bfloat162float(o_lo[row * ldo + c]);
       acc += dO[row * lddo + c] * o;
     }
-    acc = wsum(acc);
+    acc = warp_sum(acc);
     if (lane == 0) delta[((long long)b * H + h) * N + i] = acc;
   }
 }
 
-// ---- adjoint of the bilinear resize (align_corners = False) -------------------------------------------------------------
-__device__ __forceinline__ void bilin_coord_t(int d, float scale, int in_size, int& i0, int& i1, float& l1) {
-  float s = scale * (d + 0.5f) - 0.5f;
-  if (s < 0.f) s = 0.f;
-  i0 = (int)s;
-  if (i0 > in_size - 1) i0 = in_size - 1;
-  i1 = i0 + (i0 < in_size - 1 ? 1 : 0);
-  l1 = s - (float)i0;
-}
-
+// ---- adjoint of the bilinear resize (align_corners = False, bilin_coord) -----------------------------------------------
 // dy NHWC [B,H2,W2,C] (nchw = 0: one warp per output pixel, lanes over channels) or NCHW [B,C,H2,W2] (nchw = 1: one
 // thread per output pixel, loop over channels); dx NHWC [B,h,w,C] accumulated with atomics (zeroed by the caller).
 __global__ void __launch_bounds__(256)
@@ -458,8 +404,8 @@ bilinear_bwd_kernel(const float* __restrict__ dy, long long lddy, int nchw, int 
   const int x = (int)(gpix % W2), y = (int)((gpix / W2) % H2), b = (int)(gpix / ((long long)W2 * H2));
   int y0, y1, x0, x1;
   float ly, lx;
-  bilin_coord_t(y, sy, h, y0, y1, ly);
-  bilin_coord_t(x, sx, w, x0, x1, lx);
+  bilin_coord(y, sy, h, y0, y1, ly);
+  bilin_coord(x, sx, w, x0, x1, lx);
   const float hy = 1.f - ly, hx = 1.f - lx;
   float* ob = dx + (long long)b * h * w * lddx;
   float* p00 = ob + ((long long)y0 * w + x0) * lddx;
@@ -504,8 +450,7 @@ gate_bwd_kernel(const float* __restrict__ x, long long ldx, long long x_group_ro
   if (gp >= (long long)B * P) return;
   const int lane = threadIdx.x & 31;
   const int b = (int)(gp / P), pix = (int)(gp % P);
-  const int py = pix / gw, px = pix % gw;
-  const int win = (py / (gh / nh)) * nw + px / (gw / nw);
+  const int win = chan_window(pix, gh, gw, nh, nw);
   const int dh = C / H;
   const long long xrow = (long long)b * x_group_rows + x_row_offset + pix;
   const float* xr = x + xrow * ldx;
@@ -523,7 +468,7 @@ gate_bwd_kernel(const float* __restrict__ x, long long ldx, long long x_group_ro
       acc += a * xv;
       dxr[c] += a * (1.f + g) + e * (1.f + cl[(long long)c * (nh * nw)]);
     }
-    acc = wsum(acc);
+    acc = warp_sum(acc);
     if (lane == 0) d_plog[li] += acc;
   }
 }
@@ -567,8 +512,7 @@ chan_logits_bwd_kernel(const float* __restrict__ d_rc, const float* __restrict__
   if (gp >= (long long)B * P) return;
   const int lane = threadIdx.x & 31;
   const int b = (int)(gp / P), pix = (int)(gp % P);
-  const int py = pix / gw, px = pix % gw;
-  const int win = (py / (gh / nh)) * nw + px / (gw / nw);
+  const int win = chan_window(pix, gh, gw, nh, nw);
   const int nwin = nh * nw;
   const long long row = (long long)b * N + T + pix;
   for (int t = 0; t < T; ++t) {
@@ -582,7 +526,7 @@ chan_logits_bwd_kernel(const float* __restrict__ d_rc, const float* __restrict__
       acc += g * xv;
       dxn[row * lddx + c] += g * cpv;
     }
-    acc = wsum(acc);
+    acc = warp_sum(acc);
     if (lane == 0) dcp[((long long)b * T + t) * P + pix] = acc;
   }
 }
@@ -599,7 +543,7 @@ ctr_dw_kernel(const float* __restrict__ dnew, const float* __restrict__ F, int T
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   for (long long r = (long long)blockIdx.z * 8 + warp; r < rows_per_batch; r += (long long)gridDim.z * 8)
     for (int c = lane; c < C; c += 32) acc += a[r * ld + c] * f[r * ld + c];
-  acc = wsum(acc);
+  acc = warp_sum(acc);
   __shared__ float sh[8];
   if (lane == 0) sh[warp] = acc;
   __syncthreads();
@@ -715,10 +659,7 @@ im2col_patch_t_kernel(const float* __restrict__ img, int B, int Cin, int H, int 
   const int kx = row % patch, ky = (row / patch) % patch, c = row / (patch * patch);
   const int px = (int)(col % gw), py = (int)((col / gw) % gh), b = (int)(col / ((long long)gw * gh));
   const float v = img[(((long long)b * Cin + c) * H + py * patch + ky) * W + px * patch + kx];
-  __nv_bfloat16 h, l;
-  split_bf16(v, h, l);
-  hi[(long long)row * ldo + col] = h;
-  if (lo) lo[(long long)row * ldo + col] = l;
+  store_split({hi, lo, ldo}, row, col, v);
 }
 
 // ---- optimiser ----------------------------------------------------------------------------------------------------------
@@ -727,7 +668,7 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g,
   float acc = 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     acc += g[i] * g[i];
-  acc = wsum(acc);
+  acc = warp_sum(acc);
   __shared__ float sh[8];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   if (lane == 0) sh[warp] = acc;
