@@ -416,8 +416,8 @@ class _Plan(Plan):
                 self.cols = S(B * P, self.patch * self.patch * bb.in_chans)
                 self.qkv = S(B * N, 3 * C)
                 self.ao = S(B * N, C)
-                self.ws_qkv = ops.workspace(ops.workspace_bytes(ops._L.OP_LN_QKV, rows=B * N, Cdim=C, nsplit=ns), device)
-                self.ws_mlp = ops.workspace(ops.workspace_bytes(ops._L.OP_LN_MLP_RESIDUAL, rows=B * N, Cdim=C,
+                self.ws_qkv = ops.workspace(ops.workspace_bytes(ops.OP_LN_QKV, rows=B * N, Cdim=C, nsplit=ns), device)
+                self.ws_mlp = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * N, Cdim=C,
                                                                 hidden=bb.blocks[0].mlp.fc1.out_features, nsplit=ns),
                                             device)
             if mode != "invpt":
@@ -476,7 +476,7 @@ class _Plan(Plan):
                 s.P = S(B * 2 * s.Lq, s.Tk, zero=True)
                 s.ao = S(B * s.Lq, Ci)
                 s.a32 = z(B * s.Lq, Ci)
-                s.ws_mlp = ops.workspace(ops.workspace_bytes(ops._L.OP_LN_MLP_RESIDUAL, rows=B * T * h * w, Cdim=Ci,
+                s.ws_mlp = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * T * h * w, Cdim=Ci,
                                                              hidden=4 * Ci, nsplit=ns), device)
                 if i == 0:
                     s.ln32 = z(T * B * h * w, Ci)

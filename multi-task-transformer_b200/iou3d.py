@@ -7,7 +7,7 @@ how many boxes survived, which `nms_gpu` does once to size its result exactly li
 import torch
 
 from . import lib as _L
-from .ops import _ptr, _stream
+from .ops import _launch, _ptr
 
 
 def _boxes(t):
@@ -32,8 +32,7 @@ def _pairwise(boxes_a, boxes_b, mode):
     out = a.new_zeros((a.shape[0], b.shape[0]))
     if out.numel() == 0:
         return out
-    rc = _L.load().mtt_boxes_bev_pairwise(_ptr(a), a.shape[0], _ptr(b), b.shape[0], mode, _ptr(out), _stream())
-    _L.check(rc, "mtt_boxes_bev_pairwise")
+    _launch("mtt_boxes_bev_pairwise", _ptr(a), a.shape[0], _ptr(b), b.shape[0], mode, _ptr(out))
     return out
 
 
@@ -46,9 +45,8 @@ def nms_sorted(boxes_sorted, thresh, rotated=True):
     num = torch.zeros(1, dtype=torch.int32, device=b.device)
     nbytes = int(_L.load().mtt_nms_workspace_bytes(n))
     ws = torch.empty(nbytes // 8 + 1, dtype=torch.int64, device=b.device)
-    rc = _L.load().mtt_nms_bev(_ptr(b), n, float(thresh), 1 if rotated else 0, _ptr(keep), _ptr(num), _ptr(ws),
-                               ws.numel() * 8, _stream())
-    _L.check(rc, "mtt_nms_bev")
+    _launch("mtt_nms_bev", _ptr(b), n, float(thresh), 1 if rotated else 0, _ptr(keep), _ptr(num), _ptr(ws),
+            ws.numel() * 8)
     return keep[:n], num
 
 

@@ -11,7 +11,7 @@ import torch
 import torch.nn as nn
 
 from . import lib as _L
-from .ops import _ptr, _stream
+from .ops import _launch, _ptr
 
 
 def _ws(device):
@@ -31,9 +31,8 @@ class _CE(torch.autograd.Function):
         B, Cc, H, W = x.shape
         assert y.numel() == B * H * W, "label must be [B,1,H,W]"
         loss, ws = torch.empty((), device=x.device), _ws(x.device)
-        rc = _L.load().mtt_loss_cross_entropy(_ptr(x), _ptr(y), B, Cc, H, W, float(ignore_index), int(balanced), _ptr(loss),
-                                              _ptr(ws), _stream())
-        _L.check(rc, "mtt_loss_cross_entropy")
+        _launch("mtt_loss_cross_entropy", _ptr(x), _ptr(y), B, Cc, H, W, float(ignore_index), int(balanced), _ptr(loss),
+                _ptr(ws))
         ctx.save_for_backward(x, y, ws)
         ctx.args = (float(ignore_index), int(balanced), out.dtype)
         return loss
@@ -44,9 +43,8 @@ class _CE(torch.autograd.Function):
         B, Cc, H, W = x.shape
         d = torch.empty_like(x)
         gs = g.detach().float().contiguous()
-        rc = _L.load().mtt_loss_cross_entropy_grad(_ptr(x), _ptr(y), B, Cc, H, W, ctx.args[0], ctx.args[1], _ptr(gs),
-                                                   _ptr(d), _ptr(ws), _stream())
-        _L.check(rc, "mtt_loss_cross_entropy_grad")
+        _launch("mtt_loss_cross_entropy_grad", _ptr(x), _ptr(y), B, Cc, H, W, ctx.args[0], ctx.args[1], _ptr(gs),
+                _ptr(d), _ptr(ws))
         return d.to(ctx.args[2]), None, None, None
 
 
@@ -57,9 +55,8 @@ class _BCE(torch.autograd.Function):
         assert x.numel() == y.numel()
         hed = pos_weight is None
         loss, ws = torch.empty((), device=x.device), _ws(x.device)
-        rc = _L.load().mtt_loss_balanced_bce(_ptr(x), _ptr(y), x.numel(), float(ignore_index),
-                                             0.0 if hed else float(pos_weight), int(hed), _ptr(loss), _ptr(ws), _stream())
-        _L.check(rc, "mtt_loss_balanced_bce")
+        _launch("mtt_loss_balanced_bce", _ptr(x), _ptr(y), x.numel(), float(ignore_index),
+                0.0 if hed else float(pos_weight), int(hed), _ptr(loss), _ptr(ws))
         ctx.save_for_backward(x, y, ws)
         ctx.args = (float(ignore_index), 0.0 if hed else float(pos_weight), int(hed), out.dtype)
         return loss
@@ -69,9 +66,8 @@ class _BCE(torch.autograd.Function):
         x, y, ws = ctx.saved_tensors
         d = torch.empty_like(x)
         gs = g.detach().float().contiguous()
-        rc = _L.load().mtt_loss_balanced_bce_grad(_ptr(x), _ptr(y), x.numel(), ctx.args[0], ctx.args[1], ctx.args[2],
-                                                  _ptr(gs), _ptr(d), _ptr(ws), _stream())
-        _L.check(rc, "mtt_loss_balanced_bce_grad")
+        _launch("mtt_loss_balanced_bce_grad", _ptr(x), _ptr(y), x.numel(), ctx.args[0], ctx.args[1], ctx.args[2],
+                _ptr(gs), _ptr(d), _ptr(ws))
         return d.to(ctx.args[3]), None, None, None
 
 
@@ -82,9 +78,8 @@ class _L1(torch.autograd.Function):
         B, Cc, H, W = x.shape
         assert tuple(y.shape) == tuple(x.shape)
         loss, ws = torch.empty((), device=x.device), _ws(x.device)
-        rc = _L.load().mtt_loss_l1(_ptr(x), _ptr(y), B, Cc, H, W, float(ignore_index), int(use_ignore), int(normalize),
-                                   _ptr(loss), _ptr(ws), _stream())
-        _L.check(rc, "mtt_loss_l1")
+        _launch("mtt_loss_l1", _ptr(x), _ptr(y), B, Cc, H, W, float(ignore_index), int(use_ignore), int(normalize),
+                _ptr(loss), _ptr(ws))
         ctx.save_for_backward(x, y, ws)
         ctx.args = (float(ignore_index), int(use_ignore), int(normalize), out.dtype)
         return loss
@@ -95,9 +90,8 @@ class _L1(torch.autograd.Function):
         B, Cc, H, W = x.shape
         d = torch.empty_like(x)
         gs = g.detach().float().contiguous()
-        rc = _L.load().mtt_loss_l1_grad(_ptr(x), _ptr(y), B, Cc, H, W, ctx.args[0], ctx.args[1], ctx.args[2], _ptr(gs),
-                                        _ptr(d), _ptr(ws), _stream())
-        _L.check(rc, "mtt_loss_l1_grad")
+        _launch("mtt_loss_l1_grad", _ptr(x), _ptr(y), B, Cc, H, W, ctx.args[0], ctx.args[1], ctx.args[2], _ptr(gs),
+                _ptr(d), _ptr(ws))
         return d.to(ctx.args[3]), None, None, None, None
 
 

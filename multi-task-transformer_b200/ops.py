@@ -11,14 +11,33 @@ import torch
 from . import lib as _L
 
 ACT_NONE, ACT_GELU, ACT_RELU = _L.ACT_NONE, _L.ACT_GELU, _L.ACT_RELU
+OP_LN_QKV, OP_ATTN_FWD, OP_PROJ_RESIDUAL, OP_LN_MLP_RESIDUAL, OP_CHAN_PROMPT_LOGITS = (
+    _L.OP_LN_QKV, _L.OP_ATTN_FWD, _L.OP_PROJ_RESIDUAL, _L.OP_LN_MLP_RESIDUAL, _L.OP_CHAN_PROMPT_LOGITS)
+OP_GATED_CONV1X1, OP_CONV3X3_BN_ACT, OP_BILINEAR_UP, OP_INVPT_ATTN, OP_LAYERNORM = (
+    _L.OP_GATED_CONV1X1, _L.OP_CONV3X3_BN_ACT, _L.OP_BILINEAR_UP, _L.OP_INVPT_ATTN, _L.OP_LAYERNORM)
 
 
 def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _launch(name, *args):
+    """Call the library's entry point `name` with `args` and the current stream; RuntimeError when it fails."""
+    _L.check(getattr(_L.load(), name)(*args, _stream()), name)
+
+
+def device_check():
+    """RuntimeError unless the current device can run the library's kernels."""
+    _L.check(_L.load().mtt_device_check(), "mtt_device_check")
+
+
 def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+
+
+def _planes(s, row=0, col=0, lo=True):
+    """Split.planes() of an optional operand: NULL planes and ld 0 for None."""
+    return (0, 0, 0) if s is None else s.planes(row, col, lo)
 
 
 def round_up(x, m):
@@ -59,6 +78,12 @@ class Split:
     def lo(self):
         return self.buf[1] if self.nsplit == 2 else None
 
+    def planes(self, row=0, col=0, lo=True):
+        """(hi address, lo address or 0, ld) from element (row, col) on: the form the C ABI takes a split operand in.
+        The lo address is 0 when there is one plane or lo is False."""
+        hi = self.buf.data_ptr() + 2 * (row * self.ld + col)
+        return hi, (hi + 2 * self.buf.stride(0) if lo and self.nsplit == 2 else 0), self.ld
+
     def float(self):
         """Reconstruct the fp32 values (testing / debugging only)."""
         x = self.buf[0, :, : self.cols].float()
@@ -74,10 +99,7 @@ def split_f32(x, nsplit=2, cols_pad=None, out=None):
     cols_pad = cols if cols_pad is None else cols_pad
     if out is None:
         out = Split(rows, cols_pad, x.device, nsplit, ld=round_up(cols_pad, 8))
-    lib = _L.load()
-    rc = lib.mtt_split_f32(_ptr(x), x.stride(0), _ptr(out.hi), _ptr(out.lo), out.ld, rows, cols,
-                           cols_pad, _stream())
-    _L.check(rc, "mtt_split_f32")
+    _launch("mtt_split_f32", _ptr(x), x.stride(0), *out.planes(), rows, cols, cols_pad)
     return out
 
 
@@ -85,14 +107,8 @@ def layernorm(x, gamma, beta, eps, out_f32=None, out_split=None):
     """x fp32 [rows, cols] -> out_f32 (fp32 tensor) and/or out_split (Split)."""
     assert x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1
     rows, cols = x.shape
-    lib = _L.load()
-    rc = lib.mtt_layernorm(
-        _ptr(x), x.stride(0), _ptr(gamma), _ptr(beta), float(eps),
-        _ptr(out_f32), out_f32.stride(0) if out_f32 is not None else 0,
-        _ptr(out_split.hi) if out_split is not None else None,
-        _ptr(out_split.lo) if out_split is not None else None,
-        out_split.ld if out_split is not None else 0, rows, cols, _stream())
-    _L.check(rc, "mtt_layernorm")
+    _launch("mtt_layernorm", _ptr(x), x.stride(0), _ptr(gamma), _ptr(beta), float(eps),
+            _ptr(out_f32), out_f32.stride(0) if out_f32 is not None else 0, *_planes(out_split), rows, cols)
 
 
 def gemm(a, w, *, sk_ws=None, **kw):
@@ -108,8 +124,7 @@ def gemm(a, w, *, sk_ws=None, **kw):
     _fill_gemm_desc(d, a, w, **kw)
     if sk_ws is not None:
         d.sk_ws, d.sk_ws_bytes = sk_ws.data_ptr(), sk_ws.numel()
-    rc = _L.load().mtt_gemm(C.byref(d), _stream())
-    _L.check(rc, "mtt_gemm")
+    _launch("mtt_gemm", C.byref(d))
 
 
 def gemm_grouped(calls):
@@ -118,8 +133,7 @@ def gemm_grouped(calls):
     arr = (_L.GemmDesc * len(calls))()
     for d, (a, w, kw) in zip(arr, calls):
         _fill_gemm_desc(d, a, w, **kw)
-    rc = _L.load().mtt_gemm_grouped(arr, len(calls), _stream())
-    _L.check(rc, "mtt_gemm_grouped")
+    _launch("mtt_gemm_grouped", arr, len(calls))
 
 
 def gemm_splitk(a, w, partial, out_f32, *, K, bias=None, chunks):
@@ -134,9 +148,8 @@ def gemm_splitk(a, w, partial, out_f32, *, K, bias=None, chunks):
         calls.append((a, w, dict(M=M, N=N, K=kk, out_f32=partial[len(calls)], a_col_offset=k0, w_col_offset=k0)))
         k0 += kk
     gemm_grouped(calls) if len({c[2]["K"] for c in calls}) == 1 else [gemm(c[0], c[1], **c[2]) for c in calls]
-    rc = _L.load().mtt_sum_partials(_ptr(partial), len(calls), M, N, partial.stride(-2), _ptr(bias), _ptr(out_f32),
-                                    out_f32.stride(-2), _stream())
-    _L.check(rc, "mtt_sum_partials")
+    _launch("mtt_sum_partials", _ptr(partial), len(calls), M, N, partial.stride(-2), _ptr(bias), _ptr(out_f32),
+            out_f32.stride(-2))
 
 
 def _fill_gemm_desc(d, a, w, *, M=None, N=None, K=None, bias=None, act=ACT_NONE, residual=None, res_row_mod=0,
@@ -145,10 +158,8 @@ def _fill_gemm_desc(d, a, w, *, M=None, N=None, K=None, bias=None, act=ACT_NONE,
     """w_row_offset / out_row_offset: first row of the B operand / of the split output (pointer offsets): lets one
     buffer hold the operands of several (batch, head) problems of a grouped launch."""
     nsplit = min(a.nsplit, w.nsplit)
-    aoff = 2 * (a_row_offset * a.ld + a_col_offset)
-    d.a_hi, d.a_lo, d.lda = a.hi.data_ptr() + aoff, (a.lo.data_ptr() + aoff if nsplit == 2 else 0), a.ld
-    woff = 2 * (w_row_offset * w.ld + w_col_offset)
-    d.b_hi, d.b_lo, d.ldb = w.hi.data_ptr() + woff, (w.lo.data_ptr() + woff if nsplit == 2 else 0), w.ld
+    d.a_hi, d.a_lo, d.lda = a.planes(a_row_offset, a_col_offset, lo=nsplit == 2)
+    d.b_hi, d.b_lo, d.ldb = w.planes(w_row_offset, w_col_offset, lo=nsplit == 2)
     d.M = a.rows if M is None else M
     d.N = w.rows if N is None else N
     d.K = a.cols if K is None else K
@@ -168,10 +179,7 @@ def _fill_gemm_desc(d, a, w, *, M=None, N=None, K=None, bias=None, act=ACT_NONE,
         assert out_f32.dtype == torch.float32 and out_f32.stride(-1) == 1
         d.out_f32, d.ldo_f32 = out_f32.data_ptr(), out_f32.stride(-2)
     if out_split is not None:
-        ooff = 2 * (out_row_offset * out_split.ld + out_col_offset)
-        d.out_hi = out_split.hi.data_ptr() + ooff
-        d.out_lo = (out_split.lo.data_ptr() + ooff) if out_split.nsplit == 2 else 0
-        d.ldo_bf = out_split.ld
+        d.out_hi, d.out_lo, d.ldo_bf = out_split.planes(out_row_offset, out_col_offset)
         if nsplit == 2 and out_split.nsplit != 2:
             raise ValueError("nsplit=2 GEMM needs a 2-plane split output")
     if regroup is not None:
@@ -187,15 +195,14 @@ def attention(qkv, out, *, B, N, H, scale, prompt_logits=None, T=0):
     d = _L.AttnDesc()
     nsplit = min(qkv.nsplit, out.nsplit)
     assert qkv.ld == 3 * H * 64 and out.ld == H * 64
-    d.qkv_hi, d.qkv_lo = qkv.hi.data_ptr(), (qkv.lo.data_ptr() if nsplit == 2 else 0)
-    d.out_hi, d.out_lo = out.hi.data_ptr(), (out.lo.data_ptr() if out.nsplit == 2 else 0)   # lo written in either mode
+    d.qkv_hi, d.qkv_lo, _ = qkv.planes(lo=nsplit == 2)
+    d.out_hi, d.out_lo, _ = out.planes()   # lo written in either mode
     if prompt_logits is not None:
         assert prompt_logits.dtype == torch.float32 and prompt_logits.is_contiguous()
         assert tuple(prompt_logits.shape) == (B, H, T, N)
         d.prompt_logits = prompt_logits.data_ptr()
     d.B, d.N, d.H, d.T, d.nsplit, d.scale = B, N, H, T, nsplit, float(scale)
-    rc = _L.load().mtt_attention(C.byref(d), _stream())
-    _L.check(rc, "mtt_attention")
+    _launch("mtt_attention", C.byref(d))
 
 
 def streamk_workspace(device):
@@ -246,23 +253,18 @@ def im2col_patch(img, patch, out):
     """img fp32 NCHW -> out Split [B*P, Cin*patch*patch]."""
     assert img.dtype == torch.float32 and img.is_contiguous()
     B, Cin, H, W = img.shape
-    rc = _L.load().mtt_im2col_patch(_ptr(img), B, Cin, H, W, patch, _ptr(out.hi), _ptr(out.lo), out.ld,
-                                    _stream())
-    _L.check(rc, "mtt_im2col_patch")
+    _launch("mtt_im2col_patch", _ptr(img), B, Cin, H, W, patch, *out.planes())
 
 
 def broadcast_rows(src, dst, B, group_rows):
     """dst[(b*group_rows + t), :] = src[t, :] for t < T; dst fp32 [B*group_rows, ld]."""
     T, Cc = src.shape
     assert src.is_contiguous() and src.dtype == torch.float32 and dst.dtype == torch.float32
-    rc = _L.load().mtt_broadcast_rows(_ptr(src), _ptr(dst), B, T, Cc, group_rows, dst.stride(0), _stream())
-    _L.check(rc, "mtt_broadcast_rows")
+    _launch("mtt_broadcast_rows", _ptr(src), _ptr(dst), B, T, Cc, group_rows, dst.stride(0))
 
 
 def chan_logits(cp, xn, out, *, B, N, T, Cdim, gh, gw, nh, nw):
-    rc = _L.load().mtt_chan_logits(_ptr(cp), _ptr(xn.hi), _ptr(xn.lo), xn.ld, B, N, T, Cdim, gh, gw, nh, nw,
-                                   _ptr(out), _stream())
-    _L.check(rc, "mtt_chan_logits")
+    _launch("mtt_chan_logits", _ptr(cp), *xn.planes(), B, N, T, Cdim, gh, gw, nh, nw, _ptr(out))
 
 
 def gate_split(x, x_group_rows, x_row_offset, prompt_logits, chan_lg, task, ys, yc, *, B, T, N, H, Cdim, gh,
@@ -270,35 +272,24 @@ def gate_split(x, x_group_rows, x_row_offset, prompt_logits, chan_lg, task, ys, 
     """Gate the patch map for tasks [task, task + ntasks) in one pass; ys / yc are the Splits of the FIRST task, task k's
     planes live k * task_stride elements further on (one task: plain Splits)."""
     assert x.dtype == torch.float32 and x.stride(-1) == 1 and ys.ld == yc.ld
-    rc = _L.load().mtt_gate_split(_ptr(x), x.stride(-2), x_group_rows, x_row_offset, _ptr(prompt_logits),
-                                  _ptr(chan_lg), task, ntasks, B, T, N, H, Cdim, gh, gw, nh, nw, _ptr(ys.hi),
-                                  _ptr(ys.lo), _ptr(yc.hi), _ptr(yc.lo), ys.ld, task_stride, _stream())
-    _L.check(rc, "mtt_gate_split")
+    _launch("mtt_gate_split", _ptr(x), x.stride(-2), x_group_rows, x_row_offset, _ptr(prompt_logits), _ptr(chan_lg),
+            task, ntasks, B, T, N, H, Cdim, gh, gw, nh, nw, *ys.planes()[:2], *yc.planes()[:2], ys.ld, task_stride)
 
 
 def ctr_weights(prompt_logits, w0, b0, w2, b2, out, *, B, H, T, N):
-    rc = _L.load().mtt_ctr_weights(_ptr(prompt_logits), B, H, T, N, _ptr(w0), _ptr(b0), _ptr(w2), _ptr(b2),
-                                   _ptr(out), _stream())
-    _L.check(rc, "mtt_ctr_weights")
+    _launch("mtt_ctr_weights", _ptr(prompt_logits), B, H, T, N, _ptr(w0), _ptr(b0), _ptr(w2), _ptr(b2), _ptr(out))
 
 
 def ctr_mix(F, w, acc, *, T, M, Cdim, ld, rows_per_batch, accumulate):
-    rc = _L.load().mtt_ctr_mix(_ptr(F), _ptr(w), _ptr(acc), T, M, Cdim, ld, rows_per_batch,
-                               1 if accumulate else 0, _stream())
-    _L.check(rc, "mtt_ctr_mix")
+    _launch("mtt_ctr_mix", _ptr(F), _ptr(w), _ptr(acc), T, M, Cdim, ld, rows_per_batch, 1 if accumulate else 0)
 
 
 def bilinear(x, ld_in, B, h, w, Cdim, H2, W2, *, out_f32=None, out_split=None, out_nchw=None,
              accumulate=False, in_batch_rows=0, in_row_offset=0, out_batch_rows=0, out_row_offset=0):
     """x: NHWC fp32 [B*h*w, ld_in] -> NHWC fp32 / NHWC Split / NCHW fp32 [B,C,H2,W2]."""
-    rc = _L.load().mtt_bilinear(
-        _ptr(x), ld_in, B, h, w, Cdim, H2, W2, _ptr(out_f32),
-        out_f32.stride(-2) if out_f32 is not None else 0,
-        _ptr(out_split.hi) if out_split is not None else None,
-        _ptr(out_split.lo) if out_split is not None else None,
-        out_split.ld if out_split is not None else 0, _ptr(out_nchw), 1 if accumulate else 0,
-        in_batch_rows, in_row_offset, out_batch_rows, out_row_offset, _stream())
-    _L.check(rc, "mtt_bilinear")
+    _launch("mtt_bilinear", _ptr(x), ld_in, B, h, w, Cdim, H2, W2, _ptr(out_f32),
+            out_f32.stride(-2) if out_f32 is not None else 0, *_planes(out_split), _ptr(out_nchw),
+            1 if accumulate else 0, in_batch_rows, in_row_offset, out_batch_rows, out_row_offset)
 
 
 POSTPROC_KIND = {"semseg": 0, "human_parts": 0, "edge": 1, "sal": 2, "normals": 3, "depth": 4}
@@ -310,9 +301,7 @@ def bilinear_postproc(x, ld_in, B, h, w, Cdim, H2, W2, kind, out):
     i64 = out if kind == 0 else None
     f32 = None if kind == 0 else out
     assert out.is_contiguous() and out.dtype == (torch.int64 if kind == 0 else torch.float32)
-    rc = _L.load().mtt_bilinear_postproc(_ptr(x), ld_in, B, h, w, Cdim, H2, W2, kind, _ptr(i64), _ptr(f32),
-                                         _stream())
-    _L.check(rc, "mtt_bilinear_postproc")
+    _launch("mtt_bilinear_postproc", _ptr(x), ld_in, B, h, w, Cdim, H2, W2, kind, _ptr(i64), _ptr(f32))
 
 
 METER_CONFUSION, METER_SALIENCY, METER_NORMALS, METER_DEPTH, METER_EDGE = (
@@ -329,7 +318,7 @@ def meter_state_bytes(kind, n=0):
 
 
 def meter_reset(state, kind, n=0):
-    _L.check(_L.load().mtt_meter_reset(_ptr(state), int(kind), int(n), _stream()), "mtt_meter_reset")
+    _launch("mtt_meter_reset", _ptr(state), int(kind), int(n))
 
 
 def _meter_inputs(what, pred, pred_dtype, pred_shape, label, label_channels, state, int64_labels=False):
@@ -360,26 +349,21 @@ def meter_confusion_update(pred, label, n_classes, ignore_index, state):
     B, H, W = _meter_inputs("meter_confusion_update", pred, torch.int64, lambda b, h, w: (b, h, w), label, 1, state,
                             int64_labels=True)
     fn = "mtt_meter_confusion_update_i64" if label.dtype == torch.int64 else "mtt_meter_confusion_update"
-    rc = getattr(_L.load(), fn)(_ptr(pred), _ptr(label), B, H, W, int(n_classes), float(ignore_index), _ptr(state),
-                                _stream())
-    _L.check(rc, fn)
+    _launch(fn, _ptr(pred), _ptr(label), B, H, W, int(n_classes), float(ignore_index), _ptr(state))
 
 
 def meter_saliency_update(pred, label, thresholds, ignore_index, state):
     """pred fp32 [B,H,W] (255 * probability), label fp32 [B,1,H,W], thresholds fp32 on the device."""
     B, H, W = _meter_inputs("meter_saliency_update", pred, torch.float32, lambda b, h, w: (b, h, w), label, 1, state)
     assert thresholds.is_cuda and thresholds.dtype == torch.float32 and thresholds.is_contiguous()
-    rc = _L.load().mtt_meter_saliency_update(_ptr(pred), _ptr(label), B, H, W, _ptr(thresholds), thresholds.numel(),
-                                             float(ignore_index), _ptr(state), _stream())
-    _L.check(rc, "mtt_meter_saliency_update")
+    _launch("mtt_meter_saliency_update", _ptr(pred), _ptr(label), B, H, W, _ptr(thresholds), thresholds.numel(),
+            float(ignore_index), _ptr(state))
 
 
 def meter_normals_update(pred, label, ignore_index, state):
     """pred fp32 [B,H,W,3] (predict()'s normals), label fp32 [B,3,H,W]."""
     B, H, W = _meter_inputs("meter_normals_update", pred, torch.float32, lambda b, h, w: (b, h, w, 3), label, 3, state)
-    rc = _L.load().mtt_meter_normals_update(_ptr(pred), _ptr(label), B, H, W, float(ignore_index), _ptr(state),
-                                            _stream())
-    _L.check(rc, "mtt_meter_normals_update")
+    _launch("mtt_meter_normals_update", _ptr(pred), _ptr(label), B, H, W, float(ignore_index), _ptr(state))
 
 
 def meter_depth_update(pred, label, state, *, min_depth=None, max_depth=None, ignore_index=255):
@@ -388,19 +372,16 @@ def meter_depth_update(pred, label, state, *, min_depth=None, max_depth=None, ig
     shape = (lambda b, h, w: (b, h, w, 1)) if pred.dim() == 4 else (lambda b, h, w: (b, h, w))
     B, H, W = _meter_inputs("meter_depth_update", pred, torch.float32, shape, label, 1, state)
     use_range = min_depth is not None and max_depth is not None
-    rc = _L.load().mtt_meter_depth_update(_ptr(pred), _ptr(label), B, H, W, int(use_range),
-                                          float(min_depth) if use_range else 0.0,
-                                          float(max_depth) if use_range else 0.0, float(ignore_index), _ptr(state),
-                                          _stream())
-    _L.check(rc, "mtt_meter_depth_update")
+    _launch("mtt_meter_depth_update", _ptr(pred), _ptr(label), B, H, W, int(use_range),
+            float(min_depth) if use_range else 0.0, float(max_depth) if use_range else 0.0, float(ignore_index),
+            _ptr(state))
 
 
 def meter_edge_update(pred, label, pos_weight, ignore_index, state):
     """pred fp32 [B,H,W] (255 * sigmoid), label fp32 [B,1,H,W]."""
     B, H, W = _meter_inputs("meter_edge_update", pred, torch.float32, lambda b, h, w: (b, h, w), label, 1, state)
-    rc = _L.load().mtt_meter_edge_update(_ptr(pred), _ptr(label), B, H, W, float(pos_weight), float(ignore_index),
-                                         _ptr(state), _stream())
-    _L.check(rc, "mtt_meter_edge_update")
+    _launch("mtt_meter_edge_update", _ptr(pred), _ptr(label), B, H, W, float(pos_weight), float(ignore_index),
+            _ptr(state))
 
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)   # TP/inference.py:99,107
@@ -422,8 +403,7 @@ def preprocess_image(img_u8, out_hw, *, bgr=True, mean=IMAGENET_MEAN, std=IMAGEN
     assert out.is_contiguous() and tuple(out.shape) == (B, 3, H, W) and out.dtype == torch.float32
     m3 = (ctypes.c_float * 3)(*mean)
     s3 = (ctypes.c_float * 3)(*std)
-    rc = _L.load().mtt_preprocess_image(_ptr(img_u8), B, h, w, int(bool(bgr)), m3, s3, _ptr(out), H, W, _stream())
-    _L.check(rc, "mtt_preprocess_image")
+    _launch("mtt_preprocess_image", _ptr(img_u8), B, h, w, int(bool(bgr)), m3, s3, _ptr(out), H, W)
     return out
 
 
@@ -447,9 +427,8 @@ def cityscapes_targets(label_ids, disparity, out_hw, *, semseg=None, depth=None)
     for t in (label_ids, disparity, semseg, depth):
         if t is not None and not t.is_contiguous():
             raise ValueError("cityscapes_targets: every tensor must be contiguous")
-    rc = _L.load().mtt_cityscapes_targets(_ptr(label_ids), _ptr(disparity if depth is not None else None), B, h, w, H,
-                                          W, _ptr(semseg), _ptr(depth), _stream())
-    _L.check(rc, "mtt_cityscapes_targets")
+    _launch("mtt_cityscapes_targets", _ptr(label_ids), _ptr(disparity if depth is not None else None), B, h, w, H, W,
+            _ptr(semseg), _ptr(depth))
 
 
 def augment_workspace_bytes(B):
@@ -474,7 +453,7 @@ def augment(samples, data, *, B, H, W, train, crop_hw, tasks, task_out, image_ou
     for c in range(3):
         d.mean[c], d.std[c] = mean[c], std[c]
     d.workspace, d.workspace_bytes = workspace.data_ptr(), workspace.numel() * workspace.element_size()
-    _L.check(_L.load().mtt_augment(C.byref(d), _stream()), "mtt_augment")
+    _launch("mtt_augment", C.byref(d))
 
 
 RENDER_ENCODE = {"u8": _L.RENDER_U8, "class": _L.RENDER_CLASS, "palette_bgr": _L.RENDER_PALETTE_BGR,
@@ -563,7 +542,7 @@ def render(tasks, workspace):
         d.flags = flags.data_ptr() if flags is not None else None
     if workspace.numel() * workspace.element_size() < render_workspace_bytes(1, sum(d.B for d in descs)):
         raise ValueError("render: workspace smaller than render_workspace_bytes")
-    _L.check(_L.load().mtt_render(descs, len(tasks), _ptr(workspace), _stream()), "mtt_render")
+    _launch("mtt_render", descs, len(tasks), _ptr(workspace))
 
 
 def bilinear_sum3(srcs, out, *, B, Cdim, H2, W2):
@@ -574,50 +553,36 @@ def bilinear_sum3(srcs, out, *, B, Cdim, H2, W2):
         assert t.dtype == torch.float32 and t.stride(-1) == 1
         arr[i].in_, arr[i].ld_in, arr[i].h, arr[i].w = t.data_ptr(), t.stride(-2), h, w
         arr[i].batch_rows, arr[i].row_offset = brows, roff
-    rc = _L.load().mtt_bilinear_sum3(arr, len(srcs), B, Cdim, H2, W2, _ptr(out.hi), _ptr(out.lo), out.ld,
-                                     _stream())
-    _L.check(rc, "mtt_bilinear_sum3")
+    _launch("mtt_bilinear_sum3", arr, len(srcs), B, Cdim, H2, W2, *out.planes())
 
 
 def split_rows(x, out, *, rows, cols, in_group=0, src_group=0, src_offset=0):
     """Gather fp32 rows of x (row r at (r // in_group) * src_group + src_offset + r % in_group) -> Split."""
     assert x.dtype == torch.float32 and x.stride(-1) == 1
-    rc = _L.load().mtt_split_rows(_ptr(x), x.stride(-2), in_group, src_group, src_offset, _ptr(out.hi),
-                                  _ptr(out.lo), out.ld, rows, cols, _stream())
-    _L.check(rc, "mtt_split_rows")
+    _launch("mtt_split_rows", _ptr(x), x.stride(-2), in_group, src_group, src_offset, *out.planes(), rows, cols)
 
 
 def layernorm_seg(x, gamma, beta, eps, *, rows, cols, S=1, in_group=0, src_group=0, src_offset=0,
                   seg_stride=0, out_f32=None, out_split=None, out_seg_stride=0):
     assert x.dtype == torch.float32 and x.stride(-1) == 1
-    rc = _L.load().mtt_layernorm_seg(
-        _ptr(x), x.stride(-2), in_group, src_group, src_offset, seg_stride, S, _ptr(gamma), _ptr(beta),
-        float(eps), _ptr(out_f32), out_f32.stride(-2) if out_f32 is not None else 0,
-        _ptr(out_split.hi) if out_split is not None else None,
-        _ptr(out_split.lo) if out_split is not None else None,
-        out_split.ld if out_split is not None else 0, out_seg_stride, rows, cols, _stream())
-    _L.check(rc, "mtt_layernorm_seg")
+    _launch("mtt_layernorm_seg", _ptr(x), x.stride(-2), in_group, src_group, src_offset, seg_stride, S, _ptr(gamma),
+            _ptr(beta), float(eps), _ptr(out_f32), out_f32.stride(-2) if out_f32 is not None else 0,
+            *_planes(out_split), out_seg_stride, rows, cols)
 
 
 def zero_insert(x, out, *, B, h, w, Cdim, src_group, src_offset):
     assert x.dtype == torch.float32 and x.stride(-1) == 1
-    rc = _L.load().mtt_zero_insert(_ptr(x), x.stride(-2), src_group, src_offset, B, h, w, Cdim, _ptr(out.hi),
-                                   _ptr(out.lo), out.ld, _stream())
-    _L.check(rc, "mtt_zero_insert")
+    _launch("mtt_zero_insert", _ptr(x), x.stride(-2), src_group, src_offset, B, h, w, Cdim, *out.planes())
 
 
 def dwconv3x3_s2(x, weight, bias, out, *, B, T, h, w, Cdim):
     assert x.dtype == torch.float32 and x.stride(-1) == 1 and weight.is_contiguous() and bias.is_contiguous()
-    rc = _L.load().mtt_dwconv3x3_s2(_ptr(x), x.stride(-2), B, T, h, w, Cdim, _ptr(weight), _ptr(bias),
-                                    _ptr(out.hi), _ptr(out.lo), out.ld, _stream())
-    _L.check(rc, "mtt_dwconv3x3_s2")
+    _launch("mtt_dwconv3x3_s2", _ptr(x), x.stride(-2), B, T, h, w, Cdim, _ptr(weight), _ptr(bias), *out.planes())
 
 
 def avgpool(x, out, *, BT, h, w, Cdim, s):
     assert x.dtype == torch.float32 and x.stride(-1) == 1
-    rc = _L.load().mtt_avgpool(_ptr(x), x.stride(-2), BT, h, w, Cdim, s, _ptr(out.hi), _ptr(out.lo), out.ld,
-                               _stream())
-    _L.check(rc, "mtt_avgpool")
+    _launch("mtt_avgpool", _ptr(x), x.stride(-2), BT, h, w, Cdim, s, *out.planes())
 
 
 def invpt_fuse_softmax(raw, P, *, B, Lq, Tk, scale, prev_score=None, T=0, qh=0, qw=0, fuse_w=None, fuse_b=None,
@@ -629,9 +594,8 @@ def invpt_fuse_softmax(raw, P, *, B, Lq, Tk, scale, prev_score=None, T=0, qh=0, 
         assert prev_score.is_contiguous() and fuse_w.is_contiguous()
     if score_out is not None:
         assert score_out.is_contiguous()
-    rc = _L.load().mtt_invpt_fuse_softmax(_ptr(raw), B, Lq, Tk, float(scale), _ptr(prev_score), T, qh, qw, _ptr(fuse_w),
-                                          _ptr(fuse_b), _ptr(score_out), _ptr(P.hi), _ptr(P.lo), P.ld, _stream())
-    _L.check(rc, "mtt_invpt_fuse_softmax")
+    _launch("mtt_invpt_fuse_softmax", _ptr(raw), B, Lq, Tk, float(scale), _ptr(prev_score), T, qh, qw, _ptr(fuse_w),
+            _ptr(fuse_b), _ptr(score_out), *P.planes())
 
 
 # ------------------------------------------------------------------------------------------------
@@ -644,9 +608,7 @@ def _shape(rows=0, Cdim=0, hidden=0, nsplit=2, B=0, N=0, H=0, T=0):
 
 
 def _weight(w, nsplit):
-    x = _L.Weight()
-    x.hi, x.lo, x.ld = w.hi.data_ptr(), (w.lo.data_ptr() if nsplit == 2 else 0), w.ld
-    return x
+    return _L.Weight(*w.planes(lo=nsplit == 2))
 
 
 def workspace_bytes(op, **shape):
@@ -670,30 +632,25 @@ def ln_qkv(x, gamma, beta, eps, wqkv, bias, qkv, ws):
     """qkv = LN(x) @ Wqkv^T + b (taskprompter.py:272,:199,:201); LN(x) stays in `ws` as split planes."""
     rows, Cd = x.shape
     ns = min(wqkv.nsplit, qkv.nsplit)
-    rc = _L.load().mtt_ln_qkv(_ptr(x), x.stride(0), _ptr(gamma), _ptr(beta), float(eps), C.byref(_weight(wqkv, ns)),
-                              _ptr(bias), _ptr(qkv.hi), _ptr(qkv.lo), qkv.ld, C.byref(_shape(rows, Cd, nsplit=ns)),
-                              _ptr(ws), ws.numel(), _stream())
-    _L.check(rc, "mtt_ln_qkv")
+    _launch("mtt_ln_qkv", _ptr(x), x.stride(0), _ptr(gamma), _ptr(beta), float(eps), C.byref(_weight(wqkv, ns)),
+            _ptr(bias), *qkv.planes(), C.byref(_shape(rows, Cd, nsplit=ns)), _ptr(ws), ws.numel())
 
 
 def proj_residual(ao, wproj, bias, x):
     """x += ao @ Wproj^T + b in place (taskprompter.py:212,:273,:276)."""
     rows, Cd = x.shape
     ns = min(ao.nsplit, wproj.nsplit)
-    rc = _L.load().mtt_proj_residual(_ptr(ao.hi), _ptr(ao.lo), ao.ld, C.byref(_weight(wproj, ns)), _ptr(bias), _ptr(x),
-                                     x.stride(0), C.byref(_shape(rows, Cd, nsplit=ns)), _stream())
-    _L.check(rc, "mtt_proj_residual")
+    _launch("mtt_proj_residual", *ao.planes(), C.byref(_weight(wproj, ns)), _ptr(bias), _ptr(x), x.stride(0),
+            C.byref(_shape(rows, Cd, nsplit=ns)))
 
 
 def ln_mlp_residual(x, gamma, beta, eps, w1, b1, w2, b2, ws):
     """x += fc2(gelu(fc1(LN(x)))) in place (taskprompter.py:274,:277)."""
     rows, Cd = x.shape
     ns = min(w1.nsplit, w2.nsplit)
-    rc = _L.load().mtt_ln_mlp_residual(_ptr(x), x.stride(0), _ptr(gamma), _ptr(beta), float(eps),
-                                       C.byref(_weight(w1, ns)), _ptr(b1), C.byref(_weight(w2, ns)), _ptr(b2),
-                                       C.byref(_shape(rows, Cd, hidden=w1.rows, nsplit=ns)), _ptr(ws), ws.numel(),
-                                       _stream())
-    _L.check(rc, "mtt_ln_mlp_residual")
+    _launch("mtt_ln_mlp_residual", _ptr(x), x.stride(0), _ptr(gamma), _ptr(beta), float(eps), C.byref(_weight(w1, ns)),
+            _ptr(b1), C.byref(_weight(w2, ns)), _ptr(b2), C.byref(_shape(rows, Cd, hidden=w1.rows, nsplit=ns)),
+            _ptr(ws), ws.numel())
 
 
 def gated_conv1x1(x, x_group_rows, x_row_offset, prompt_logits, chan_lg, tasks, e, chan_col, ws, *, B, T, N, H, Cdim,
@@ -706,25 +663,20 @@ def gated_conv1x1(x, x_group_rows, x_row_offset, prompt_logits, chan_lg, tasks, 
     for g, (w_spa, b_spa, w_chan, b_chan, cat) in zip(arr, tasks):
         assert cat.ld == cat0.ld
         g.w_spa, g.b_spa, g.w_chan, g.b_chan = _weight(w_spa, ns), b_spa.data_ptr(), _weight(w_chan, ns), b_chan.data_ptr()
-        g.cat_hi, g.cat_lo = cat.hi.data_ptr(), (cat.lo.data_ptr() if ns == 2 else 0)
-    rc = _L.load().mtt_gated_conv1x1(_ptr(x), x.stride(-2), x_group_rows, x_row_offset, _ptr(prompt_logits),
-                                     _ptr(chan_lg), len(tasks), arr, gh, gw, nh, nw, e, cat0.ld, chan_col,
-                                     C.byref(_shape(0, Cdim, nsplit=ns, B=B, N=N, H=H, T=T)), _ptr(ws), ws.numel(),
-                                     _stream())
-    _L.check(rc, "mtt_gated_conv1x1")
+        g.cat_hi, g.cat_lo, _ = cat.planes(lo=ns == 2)
+    _launch("mtt_gated_conv1x1", _ptr(x), x.stride(-2), x_group_rows, x_row_offset, _ptr(prompt_logits), _ptr(chan_lg),
+            len(tasks), arr, gh, gw, nh, nw, e, cat0.ld, chan_col,
+            C.byref(_shape(0, Cdim, nsplit=ns, B=B, N=N, H=H, T=T)), _ptr(ws), ws.numel())
 
 
 def conv3x3_bn_act(a, w3, b3, Cin, Cout, act, *, B, H, W, dil=1, mid=None, w_head=None, b_head=None, n_out=0,
                    out_f32=None, ws=None):
     """3x3 conv + folded BN + act on an NHWC Split (optionally followed by the fused 1x1 head -> out_f32)."""
     ns = min(a.nsplit, w3.nsplit)
-    rc = _L.load().mtt_conv3x3_bn_act(
-        _ptr(a.hi), _ptr(a.lo), a.ld, B, H, W, Cin, dil, C.byref(_weight(w3, ns)), _ptr(b3), Cout, act,
-        _ptr(mid.hi) if mid is not None else None, _ptr(mid.lo) if mid is not None else None,
-        mid.ld if mid is not None else 0, C.byref(_weight(w_head, ns)) if w_head is not None else None, _ptr(b_head),
-        n_out, _ptr(out_f32), out_f32.stride(-2) if out_f32 is not None else 0, ns, _ptr(ws),
-        ws.numel() if ws is not None else 0, _stream())
-    _L.check(rc, "mtt_conv3x3_bn_act")
+    _launch("mtt_conv3x3_bn_act", *a.planes(), B, H, W, Cin, dil, C.byref(_weight(w3, ns)), _ptr(b3), Cout, act,
+            *_planes(mid), C.byref(_weight(w_head, ns)) if w_head is not None else None, _ptr(b_head), n_out,
+            _ptr(out_f32), out_f32.stride(-2) if out_f32 is not None else 0, ns, _ptr(ws),
+            ws.numel() if ws is not None else 0)
 
 
 def pack_weight(w, nsplit):
@@ -733,8 +685,7 @@ def pack_weight(w, nsplit):
     N, K = w.shape
     out = Split(N, round_up(K, 8), w.device, nsplit)
     out.cols = K
-    rc = _L.load().mtt_pack_weight(_ptr(w), w.stride(0), N, K, nsplit, _ptr(out.hi), _ptr(out.lo), out.ld, _stream())
-    _L.check(rc, "mtt_pack_weight")
+    _launch("mtt_pack_weight", _ptr(w), w.stride(0), N, K, nsplit, *out.planes())
     return out
 
 
@@ -755,10 +706,8 @@ def pack_conv_weight(w, bias, bn, nsplit, transposed=False):
         g = b = m = v = None
         eps = 0.0
     bias = f(bias) if bias is not None else None
-    rc = _L.load().mtt_pack_conv_weight(_ptr(w), _ptr(bias), _ptr(g), _ptr(b), _ptr(m), _ptr(v), eps, N, Cin, k,
-                                        1 if transposed else 0, nsplit, _ptr(out.hi), _ptr(out.lo), out.ld,
-                                        _ptr(bias_out), _ptr(scale), _stream())
-    _L.check(rc, "mtt_pack_conv_weight")
+    _launch("mtt_pack_conv_weight", _ptr(w), _ptr(bias), _ptr(g), _ptr(b), _ptr(m), _ptr(v), eps, N, Cin, k,
+            1 if transposed else 0, nsplit, *out.planes(), _ptr(bias_out), _ptr(scale))
     return out, bias_out
 
 
@@ -767,16 +716,12 @@ def nchw_to_nhwc_split(x, out, col_offset=0):
     forwards take NCHW like the reference)."""
     assert x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 4
     B, Cd, H, W = x.shape
-    hi = C.c_void_p(out.hi.data_ptr() + 2 * col_offset)
-    lo = C.c_void_p(out.lo.data_ptr() + 2 * col_offset) if out.nsplit == 2 else C.c_void_p(0)
-    rc = _L.load().mtt_nchw_to_nhwc_split(_ptr(x), B, Cd, H, W, hi, lo, out.ld, _stream())
-    _L.check(rc, "mtt_nchw_to_nhwc_split")
+    _launch("mtt_nchw_to_nhwc_split", _ptr(x), B, Cd, H, W, *out.planes(col=col_offset))
 
 
 def nhwc_to_nchw(x, ld_in, B, Cd, H, W, out):
     assert x.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (B, Cd, H, W)
-    rc = _L.load().mtt_nhwc_to_nchw(_ptr(x), ld_in, B, Cd, H, W, _ptr(out), _stream())
-    _L.check(rc, "mtt_nhwc_to_nchw")
+    _launch("mtt_nhwc_to_nchw", _ptr(x), ld_in, B, Cd, H, W, _ptr(out))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -784,58 +729,47 @@ def nhwc_to_nchw(x, ld_in, B, Cd, H, W, out):
 # ------------------------------------------------------------------------------------------------
 def swin_window_gather(xn, pn, out, *, B, H, W, Cdim, T, ws, shift):
     """LN1 outputs xn [B*H*W, C], pn [B*T, C] (fp32) -> out: split joint window stream [B*nW*(T + ws*ws), C]."""
-    rc = _L.load().mtt_swin_window_gather(_ptr(xn), xn.stride(0), _ptr(pn), pn.stride(0), B, H, W, Cdim, T, ws, shift,
-                                          _ptr(out.hi), _ptr(out.lo), out.ld, _stream())
-    _L.check(rc, "mtt_swin_window_gather")
+    _launch("mtt_swin_window_gather", _ptr(xn), xn.stride(0), _ptr(pn), pn.stride(0), B, H, W, Cdim, T, ws, shift,
+            *out.planes())
 
 
 def swin_window_attention(qkv, out, raw, biasT, maskT, *, BW, nW, T, L, heads, scale):
     """Window attention with prompts; biasT [heads, L, L] / maskT [nW, L, L] are stored transposed ([.., key, query])."""
     Cd = out.cols
     assert biasT.is_contiguous() and (maskT is None or maskT.is_contiguous()) and raw.is_contiguous()
-    rc = _L.load().mtt_swin_window_attention(_ptr(qkv.hi), _ptr(qkv.lo), qkv.ld, BW, nW, T, L, heads, Cd // heads,
-                                             float(scale), _ptr(biasT), _ptr(maskT), _ptr(out.hi), _ptr(out.lo), out.ld,
-                                             _ptr(raw), _stream())
-    _L.check(rc, "mtt_swin_window_attention")
+    _launch("mtt_swin_window_attention", *qkv.planes(), BW, nW, T, L, heads, Cd // heads, float(scale), _ptr(biasT),
+            _ptr(maskT), *out.planes(), _ptr(raw))
 
 
 def swin_window_scatter(o32, raw, xa, x, p, logits, *, B, H, W, Cdim, T, ws, shift, heads, last):
     """proj output on the joint stream -> xa, x += xa, p += mean prompt rows (unless last), raw -> logits map."""
-    rc = _L.load().mtt_swin_window_scatter(_ptr(o32), o32.stride(0), _ptr(raw), B, H, W, Cdim, T, ws, shift, heads,
-                                           0 if last else 1, _ptr(xa), xa.stride(0), _ptr(x), x.stride(0), _ptr(p),
-                                           p.stride(0), _ptr(logits), _stream())
-    _L.check(rc, "mtt_swin_window_scatter")
+    _launch("mtt_swin_window_scatter", _ptr(o32), o32.stride(0), _ptr(raw), B, H, W, Cdim, T, ws, shift, heads,
+            0 if last else 1, _ptr(xa), xa.stride(0), _ptr(x), x.stride(0), _ptr(p), p.stride(0), _ptr(logits))
 
 
 def transpose_split(x, out, *, B, L, Cdim):
     """x fp32 [B*L, C] -> out Split [B*C, L] (per-image transpose)."""
-    rc = _L.load().mtt_transpose_split(_ptr(x), x.stride(0), B, L, Cdim, _ptr(out.hi), _ptr(out.lo), out.ld, _stream())
-    _L.check(rc, "mtt_transpose_split")
+    _launch("mtt_transpose_split", _ptr(x), x.stride(0), B, L, Cdim, *out.planes())
 
 
 def swin_chan_attention(q, kv, co32, cos, rc_out, *, B, T, Cdim, ce, nh, nw):
-    rc = _L.load().mtt_swin_chan_attention(_ptr(q), q.stride(0), _ptr(kv), kv.stride(0), B, T, Cdim, ce, nh, nw,
-                                           _ptr(co32), co32.stride(0), _ptr(cos.hi), _ptr(cos.lo), cos.ld, _ptr(rc_out),
-                                           _stream())
-    _L.check(rc, "mtt_swin_chan_attention")
+    _launch("mtt_swin_chan_attention", _ptr(q), q.stride(0), _ptr(kv), kv.stride(0), B, T, Cdim, ce, nh, nw,
+            _ptr(co32), co32.stride(0), *cos.planes(), _ptr(rc_out))
 
 
 def swin_merge_gather(x, out, *, B, H, W, Cdim):
-    rc = _L.load().mtt_swin_merge_gather(_ptr(x), x.stride(0), B, H, W, Cdim, _ptr(out), out.stride(0), _stream())
-    _L.check(rc, "mtt_swin_merge_gather")
+    _launch("mtt_swin_merge_gather", _ptr(x), x.stride(0), B, H, W, Cdim, _ptr(out), out.stride(0))
 
 
 def conv3x3_s2_maps(x, w, b, out, *, B, Cin, H, W, in_stride, in_offset, out_stride, out_offset):
     assert w.is_contiguous() and x.is_contiguous() and out.is_contiguous()
-    rc = _L.load().mtt_conv3x3_s2_maps(_ptr(x), _ptr(w), _ptr(b), B, Cin, w.shape[0], H, W, in_stride, in_offset,
-                                       out_stride, out_offset, _ptr(out), _stream())
-    _L.check(rc, "mtt_conv3x3_s2_maps")
+    _launch("mtt_conv3x3_s2_maps", _ptr(x), _ptr(w), _ptr(b), B, Cin, w.shape[0], H, W, in_stride, in_offset,
+            out_stride, out_offset, _ptr(out))
 
 
 def swin_chan_up(rc_in, w, out, *, BT, Cdim, nwin):
     assert rc_in.is_contiguous() and w.is_contiguous() and out.is_contiguous()
-    rc = _L.load().mtt_swin_chan_up(_ptr(rc_in), _ptr(w), BT, Cdim, w.shape[0], nwin, _ptr(out), _stream())
-    _L.check(rc, "mtt_swin_chan_up")
+    _launch("mtt_swin_chan_up", _ptr(rc_in), _ptr(w), BT, Cdim, w.shape[0], nwin, _ptr(out))
 
 
 # ---- training step (csrc/train_ops.cu): fp32 [rows, cols] tensors, last dim contiguous ----------------------------------
@@ -847,39 +781,36 @@ def _ld(t):
 def colsum(x, out, accumulate=False, *, rows=None, in_group=0, src_group=0, src_offset=0):
     """out[c] (+)= sum_r x[row(r), c]; row mapping as split_rows (in_group = 0: the first `rows` rows)."""
     rows = x.shape[0] if rows is None else rows
-    _L.check(_L.load().mtt_colsum(_ptr(x), _ld(x), rows, x.shape[1], in_group, src_group, src_offset, _ptr(out),
-                                  int(accumulate), _stream()), "mtt_colsum")
+    _launch("mtt_colsum", _ptr(x), _ld(x), rows, x.shape[1], in_group, src_group, src_offset, _ptr(out),
+            int(accumulate))
 
 
 def layernorm_bwd(x, dy, gamma, eps, dx, dgamma, dbeta, *, accumulate_dx=False):
     """dx (+)= d LN(x) . dy; dgamma / dbeta are ACCUMULATED (None: skip the parameter gradients)."""
     rows, cols = x.shape
     ws = torch.empty(2 * rows, dtype=torch.float32, device=x.device)
-    _L.check(_L.load().mtt_layernorm_bwd(_ptr(x), _ld(x), _ptr(dy), _ld(dy), _ptr(gamma), float(eps), rows, cols, _ptr(dx),
-                                         _ld(dx), int(accumulate_dx), _ptr(dgamma), _ptr(dbeta), _ptr(ws), _stream()),
-             "mtt_layernorm_bwd")
+    _launch("mtt_layernorm_bwd", _ptr(x), _ld(x), _ptr(dy), _ld(dy), _ptr(gamma), float(eps), rows, cols, _ptr(dx),
+            _ld(dx), int(accumulate_dx), _ptr(dgamma), _ptr(dbeta), _ptr(ws))
 
 
 def act_split(pre, act, out=None, nsplit=2):
     rows, cols = pre.shape
     if out is None:
         out = Split(rows, cols, pre.device, nsplit)
-    _L.check(_L.load().mtt_act_split(_ptr(pre), _ld(pre), rows, cols, act, _ptr(out.hi), _ptr(out.lo), out.ld, _stream()),
-             "mtt_act_split")
+    _launch("mtt_act_split", _ptr(pre), _ld(pre), rows, cols, act, *out.planes())
     return out
 
 
 def act_bwd(pre, dy, act, dx):
     rows, cols = pre.shape
-    _L.check(_L.load().mtt_act_bwd(_ptr(pre), _ld(pre), _ptr(dy), _ld(dy), rows, cols, act, _ptr(dx), _ld(dx), _stream()),
-             "mtt_act_bwd")
+    _launch("mtt_act_bwd", _ptr(pre), _ld(pre), _ptr(dy), _ld(dy), rows, cols, act, _ptr(dx), _ld(dx))
 
 
 def axpy_rows(base, src, row_scale, dst):
     """dst = base + row_scale[:, None] * src (base / row_scale may be None)."""
     rows, cols = src.shape
-    _L.check(_L.load().mtt_axpy_rows(_ptr(base), _ld(base) if base is not None else 0, _ptr(src), _ld(src),
-                                     _ptr(row_scale), rows, cols, _ptr(dst), _ld(dst), _stream()), "mtt_axpy_rows")
+    _launch("mtt_axpy_rows", _ptr(base), _ld(base) if base is not None else 0, _ptr(src), _ld(src), _ptr(row_scale),
+            rows, cols, _ptr(dst), _ld(dst))
 
 
 def transpose_planes(a, *, B=1, R=None, Ccols=None, in_batch_rows=None, out=None, side_by_side=False):
@@ -891,9 +822,7 @@ def transpose_planes(a, *, B=1, R=None, Ccols=None, in_batch_rows=None, out=None
     if out is None:
         rows, cols = (Ccols, B * R) if side_by_side else (B * Ccols, R)
         out = Split(rows, cols, a.hi.device, a.nsplit)     # pad columns are never read (TMA bounds)
-    _L.check(_L.load().mtt_transpose_planes(_ptr(a.hi), _ptr(a.lo), a.ld, in_batch_rows, B, R, Ccols, _ptr(out.hi),
-                                            _ptr(out.lo), out.ld, R if side_by_side else 0, _stream()),
-             "mtt_transpose_planes")
+    _launch("mtt_transpose_planes", *a.planes(), in_batch_rows, B, R, Ccols, *out.planes(), R if side_by_side else 0)
     return out
 
 
@@ -901,7 +830,7 @@ def bn_stats(x, sums):
     """sums [2C] = (sum x, sum x^2) over the rows of x, accumulated in float64. Keep sums float64 (TrainStep does): a
     float32 buffer receives the rounded sums, and the variance formed from those cancels in fp32 as |mean| / std grows."""
     out = sums if sums.dtype == torch.float64 else torch.empty(sums.shape, dtype=torch.float64, device=sums.device)
-    _L.check(_L.load().mtt_bn_stats(_ptr(x), _ld(x), x.shape[0], x.shape[1], _ptr(out), _stream()), "mtt_bn_stats")
+    _launch("mtt_bn_stats", _ptr(x), _ld(x), x.shape[0], x.shape[1], _ptr(out))
     if out is not sums:
         sums.copy_(out)
 
@@ -909,81 +838,70 @@ def bn_stats(x, sums):
 def bn_finalize(sums, count, eps, momentum, mean_rstd, running_mean=None, running_var=None):
     """mean_rstd [2C] fp32 from sums (float64, or float32 widened) / count, the variance formed in float64."""
     s = sums if sums.dtype == torch.float64 else sums.double()
-    _L.check(_L.load().mtt_bn_finalize(_ptr(s), float(count), s.numel() // 2, float(eps), float(momentum),
-                                       _ptr(mean_rstd), _ptr(running_mean), _ptr(running_var), _stream()), "mtt_bn_finalize")
+    _launch("mtt_bn_finalize", _ptr(s), float(count), s.numel() // 2, float(eps), float(momentum), _ptr(mean_rstd),
+            _ptr(running_mean), _ptr(running_var))
 
 
 def bn_act(x, mean_rstd, gamma, beta, act, *, out_f32=None, out_split=None):
     rows, cols = x.shape
-    _L.check(_L.load().mtt_bn_act(_ptr(x), _ld(x), rows, cols, _ptr(mean_rstd), _ptr(gamma), _ptr(beta), act,
-                                  _ptr(out_f32), _ld(out_f32) if out_f32 is not None else 0,
-                                  _ptr(out_split.hi) if out_split is not None else None,
-                                  _ptr(out_split.lo) if out_split is not None else None,
-                                  out_split.ld if out_split is not None else 0, _stream()), "mtt_bn_act")
+    _launch("mtt_bn_act", _ptr(x), _ld(x), rows, cols, _ptr(mean_rstd), _ptr(gamma), _ptr(beta), act, _ptr(out_f32),
+            _ld(out_f32) if out_f32 is not None else 0, *_planes(out_split))
 
 
 def bn_bwd_reduce(x, dy, mean_rstd, gamma, beta, act, sums):
     rows, cols = x.shape
-    _L.check(_L.load().mtt_bn_bwd_reduce(_ptr(x), _ld(x), _ptr(dy), _ld(dy), rows, cols, _ptr(mean_rstd), _ptr(gamma),
-                                         _ptr(beta), act, _ptr(sums), _stream()), "mtt_bn_bwd_reduce")
+    _launch("mtt_bn_bwd_reduce", _ptr(x), _ld(x), _ptr(dy), _ld(dy), rows, cols, _ptr(mean_rstd), _ptr(gamma),
+            _ptr(beta), act, _ptr(sums))
 
 
 def bn_bwd_apply(x, dy, mean_rstd, gamma, beta, act, sums, count, dx):
     rows, cols = x.shape
-    _L.check(_L.load().mtt_bn_bwd_apply(_ptr(x), _ld(x), _ptr(dy), _ld(dy), rows, cols, _ptr(mean_rstd), _ptr(gamma),
-                                        _ptr(beta), act, _ptr(sums), float(count), _ptr(dx), _ld(dx), _stream()),
-             "mtt_bn_bwd_apply")
+    _launch("mtt_bn_bwd_apply", _ptr(x), _ld(x), _ptr(dy), _ld(dy), rows, cols, _ptr(mean_rstd), _ptr(gamma),
+            _ptr(beta), act, _ptr(sums), float(count), _ptr(dx), _ld(dx))
 
 
 def attn_delta(dO, o, delta, *, B, N, H, head_dim):
     """delta [B*H*N] = rowdot(dO, O) per head: dO fp32 [B*N, H*head_dim], o = the forward's attention output (Split)."""
-    _L.check(_L.load().mtt_attn_delta(_ptr(dO), _ld(dO), _ptr(o.hi), _ptr(o.lo), o.ld, B, N, H, head_dim, _ptr(delta),
-                                      _stream()), "mtt_attn_delta")
+    _launch("mtt_attn_delta", _ptr(dO), _ld(dO), *o.planes(), B, N, H, head_dim, _ptr(delta))
 
 
 def attn_softmax_bwd(S, dP, delta, *, BH, N, scale, d_raw, T, ds, pt=None, dst=None):
     """S, dP fp32 [BH*N, ld] (read only), delta fp32 [BH*N] -> Splits ds [BH*N queries, >= N], and optionally pt = P^T,
     dst = dS^T [BH*N keys, >= N queries] (same ld as ds)."""
     assert (pt is None) == (dst is None) and (pt is None or pt.ld == dst.ld == ds.ld)
-    _L.check(_L.load().mtt_attn_softmax_bwd(_ptr(S), _ptr(dP), _ptr(delta), _ld(S), BH, N, float(scale), _ptr(d_raw), T, _ptr(ds.hi),
-                                            _ptr(ds.lo), _ptr(pt.hi) if pt is not None else None,
-                                            _ptr(pt.lo) if pt is not None else None,
-                                            _ptr(dst.hi) if dst is not None else None,
-                                            _ptr(dst.lo) if dst is not None else None, ds.ld, _stream()),
-             "mtt_attn_softmax_bwd")
+    _launch("mtt_attn_softmax_bwd", _ptr(S), _ptr(dP), _ptr(delta), _ld(S), BH, N, float(scale), _ptr(d_raw), T,
+            *ds.planes()[:2], *_planes(pt)[:2], *_planes(dst)[:2], ds.ld)
 
 
 def bilinear_bwd(dy, *, nchw, B, h, w, Cdim, H2, W2, dx, accumulate=False):
-    _L.check(_L.load().mtt_bilinear_bwd(_ptr(dy), 0 if nchw else _ld(dy), int(nchw), B, h, w, Cdim, H2, W2, _ptr(dx),
-                                        _ld(dx), int(accumulate), _stream()), "mtt_bilinear_bwd")
+    _launch("mtt_bilinear_bwd", _ptr(dy), 0 if nchw else _ld(dy), int(nchw), B, h, w, Cdim, H2, W2, _ptr(dx), _ld(dx),
+            int(accumulate))
 
 
 def gate_bwd(x, x_group_rows, x_row_offset, prompt_logits, chan_lg, task, dys, dyc, dx, d_prompt_logits, d_chan_lg, *, B,
              T, N, H, Cdim, gh, gw, nh, nw):
-    _L.check(_L.load().mtt_gate_bwd(_ptr(x), _ld(x), x_group_rows, x_row_offset, _ptr(prompt_logits), _ptr(chan_lg), task,
-                                    B, T, N, H, Cdim, gh, gw, nh, nw, _ptr(dys), _ptr(dyc), _ld(dys), _ptr(dx), _ld(dx),
-                                    _ptr(d_prompt_logits), _ptr(d_chan_lg), _stream()), "mtt_gate_bwd")
+    _launch("mtt_gate_bwd", _ptr(x), _ld(x), x_group_rows, x_row_offset, _ptr(prompt_logits), _ptr(chan_lg), task, B, T,
+            N, H, Cdim, gh, gw, nh, nw, _ptr(dys), _ptr(dyc), _ld(dys), _ptr(dx), _ld(dx), _ptr(d_prompt_logits),
+            _ptr(d_chan_lg))
 
 
 def chan_logits_bwd(d_rc, cp, xn, dcp, dxn, *, B, N, T, Cdim, gh, gw, nh, nw):
-    _L.check(_L.load().mtt_chan_logits_bwd(_ptr(d_rc), _ptr(cp), _ptr(xn.hi), _ptr(xn.lo), xn.ld, B, N, T, Cdim, gh, gw, nh,
-                                           nw, _ptr(dcp), _ptr(dxn), _ld(dxn), _stream()), "mtt_chan_logits_bwd")
+    _launch("mtt_chan_logits_bwd", _ptr(d_rc), _ptr(cp), *xn.planes(), B, N, T, Cdim, gh, gw, nh, nw, _ptr(dcp),
+            _ptr(dxn), _ld(dxn))
 
 
 def ctr_bwd(dnew, F, prompt_logits, w0, b0, w2, d_prompt_logits, dw0, db0, dw2, db2, *, T, M, Cdim, ld, rows_per_batch, B,
             H, N):
     ws = torch.empty(B * T * T, dtype=torch.float32, device=dnew.device)
-    _L.check(_L.load().mtt_ctr_bwd(_ptr(dnew), _ptr(F), T, M, Cdim, ld, rows_per_batch, _ptr(prompt_logits), B, H, N,
-                                   _ptr(w0), _ptr(b0), _ptr(w2), _ptr(ws), _ptr(d_prompt_logits), _ptr(dw0), _ptr(db0),
-                                   _ptr(dw2), _ptr(db2), _stream()), "mtt_ctr_bwd")
+    _launch("mtt_ctr_bwd", _ptr(dnew), _ptr(F), T, M, Cdim, ld, rows_per_batch, _ptr(prompt_logits), B, H, N, _ptr(w0),
+            _ptr(b0), _ptr(w2), _ptr(ws), _ptr(d_prompt_logits), _ptr(dw0), _ptr(db0), _ptr(dw2), _ptr(db2))
 
 
 def im2col3x3_t(x, *, B, H, W, Cdim, nsplit=2):
     """NHWC fp32 [B*H*W, C] -> Split [C*9, B*H*W]: rows (c, ky, kx)."""
     P = B * H * W
     out = Split(Cdim * 9, P, x.device, nsplit)
-    _L.check(_L.load().mtt_im2col3x3_t(_ptr(x), _ld(x), B, H, W, Cdim, _ptr(out.hi), _ptr(out.lo), out.ld, _stream()),
-             "mtt_im2col3x3_t")
+    _launch("mtt_im2col3x3_t", _ptr(x), _ld(x), B, H, W, Cdim, *out.planes())
     return out
 
 
@@ -992,17 +910,15 @@ def im2col_patch_t(img, patch, nsplit=2):
     B, Cin, H, W = img.shape
     cols = B * (H // patch) * (W // patch)
     out = Split(Cin * patch * patch, cols, img.device, nsplit)
-    _L.check(_L.load().mtt_im2col_patch_t(_ptr(img), B, Cin, H, W, patch, _ptr(out.hi), _ptr(out.lo), out.ld, _stream()),
-             "mtt_im2col_patch_t")
+    _launch("mtt_im2col_patch_t", _ptr(img), B, Cin, H, W, patch, *out.planes())
     return out
 
 
 def sumsq(g, out, accumulate=False):
-    _L.check(_L.load().mtt_sumsq(_ptr(g), g.numel(), _ptr(out), int(accumulate), _stream()), "mtt_sumsq")
+    _launch("mtt_sumsq", _ptr(g), g.numel(), _ptr(out), int(accumulate))
 
 
 def adam_step(p, g, m, v, *, lr, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, step, gnorm_sq=None, max_norm=0.0,
               grad_scale=1.0):
-    _L.check(_L.load().mtt_adam_step(_ptr(p), _ptr(g), _ptr(m), _ptr(v), p.numel(), float(lr), float(betas[0]),
-                                     float(betas[1]), float(eps), float(weight_decay), int(step), _ptr(gnorm_sq),
-                                     float(max_norm), float(grad_scale), _stream()), "mtt_adam_step")
+    _launch("mtt_adam_step", _ptr(p), _ptr(g), _ptr(m), _ptr(v), p.numel(), float(lr), float(betas[0]), float(betas[1]),
+            float(eps), float(weight_decay), int(step), _ptr(gnorm_sq), float(max_norm), float(grad_scale))

@@ -53,7 +53,7 @@ def _check_input(mod, x):
                                   "SURVEY.md section 8f N1)")
     if not x.is_cuda:
         raise RuntimeError("mtt_b200 has no CPU path: input must be a CUDA tensor on an sm_90a (H100) device")
-    ops._L.check(ops._L.load().mtt_device_check(), "mtt_device_check")
+    ops.device_check()
 
 
 class _Streams:
@@ -114,7 +114,7 @@ class Plan:
 
     def __init__(self, modules, B, device, nsplit, n_streams):
         """modules: the nn.Modules whose parameters the packed weights follow (None entries are skipped)."""
-        ops._L.check(ops._L.load().mtt_device_check(), "mtt_device_check")
+        ops.device_check()
         self.tracked = [m for m in modules if m is not None]
         self.B, self.dev, self.ns = B, torch.device(device), nsplit
         self.streams = _Streams(self.dev, n_streams)

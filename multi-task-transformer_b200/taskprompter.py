@@ -87,8 +87,8 @@ class _BlockSpace:
         self.cps = S(B * T, P)
         self.rc = z(B, T, C, self.nh, self.nw)
         # workspaces of the two LayerNorm-fronted operators; LN1's output is read back by the channel-prompt path
-        self.ws_qkv = ops.workspace(ops.workspace_bytes(ops._L.OP_LN_QKV, rows=B * N, Cdim=C, nsplit=ns), device)
-        self.ws_mlp = ops.workspace(ops.workspace_bytes(ops._L.OP_LN_MLP_RESIDUAL, rows=B * N, Cdim=C, hidden=hidden,
+        self.ws_qkv = ops.workspace(ops.workspace_bytes(ops.OP_LN_QKV, rows=B * N, Cdim=C, nsplit=ns), device)
+        self.ws_mlp = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * N, Cdim=C, hidden=hidden,
                                                         nsplit=ns), device)
         self.xn = ops.ws_split_view(self.ws_qkv, 0, B * N, C, ns)
         self.streams = streams if streams is not None else _Streams(device, max(T, 1))
@@ -510,7 +510,7 @@ class _Plan(Plan):
             self.xfin = z(B * N, C)
             # one set of decoder scratch buffers per task: the T tasks' identically shaped convolutions of a level run
             # as grouped launches
-            self.ws_gate = ops.workspace(ops.workspace_bytes(ops._L.OP_GATED_CONV1X1, rows=B * P, Cdim=C, nsplit=ns, T=T),
+            self.ws_gate = ops.workspace(ops.workspace_bytes(ops.OP_GATED_CONV1X1, rows=B * P, Cdim=C, nsplit=ns, T=T),
                                          device)
             self.cat = [S(B * P, 2 * e_pad, zero=True) for _ in range(T)]
             self.f1 = [S(B * P, f, zero=True) for _ in range(T)]

@@ -337,9 +337,9 @@ class _SwinPlan(Plan):
                 s.t1 = S(B * T, ce)
                 s.rc = z(B, T, C, self.nh, self.nw)
                 hid = layer.blocks[0].mlp.fc1.out_features
-                s.ws_mlp = ops.workspace(ops.workspace_bytes(ops._L.OP_LN_MLP_RESIDUAL, rows=B * L, Cdim=C, hidden=hid,
+                s.ws_mlp = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * L, Cdim=C, hidden=hid,
                                                              nsplit=ns), device)
-                s.ws_mlp_p = ops.workspace(ops.workspace_bytes(ops._L.OP_LN_MLP_RESIDUAL, rows=B * T, Cdim=C, hidden=hid,
+                s.ws_mlp_p = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * T, Cdim=C, hidden=hid,
                                                                nsplit=ns), device)
                 if layer.downsample is not None:
                     s.m32 = z(B * L // 4, 4 * C)
@@ -355,7 +355,7 @@ class _SwinPlan(Plan):
                 h, w = bb.resolution[il]
                 Cl = p.backbone_channels[il]
                 d = SimpleNamespace(h=h, w=w, P=h * w, C=Cl, heads=self.st[il].heads)
-                d.ws_gate = ops.workspace(ops.workspace_bytes(ops._L.OP_GATED_CONV1X1, rows=B * d.P, Cdim=Cl, nsplit=ns, T=T),
+                d.ws_gate = ops.workspace(ops.workspace_bytes(ops.OP_GATED_CONV1X1, rows=B * d.P, Cdim=Cl, nsplit=ns, T=T),
                                           device)
                 d.cat = [S(B * d.P, 2 * self.Lv_pad, zero=True) for _ in range(T)]
                 d.g32 = [z(B * d.P, self.f_ld) for _ in range(T)]
