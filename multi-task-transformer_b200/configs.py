@@ -78,6 +78,22 @@ def taskprompter_swin(name):
                           patch=4, embed_dim=128, depths=(2, 2, 18, 2), heads=(4, 8, 16, 32), window=12,
                           img_ds_ratio=0.75, level_embed_dim=256, f=450, chan_embed_dim=256, chan_nheads=1,
                           head="deconv", dd_label_map_size=(512, 1024)),
+        # ---- three tasks with '3ddet' (its detection head is the caller's module; num_output["3ddet"] only sizes the
+        # oracle's dense stand-in parameters, which the fixtures drop)
+        # tiny: 64x128, window 6 (shift 3) padded to 18x36 / 12x18, then clipped to 4 and 2; 2x2 channel windows
+        "tps_tiny3d": dict(tasks=["semseg", "depth", "3ddet"], num_output={"semseg": 5, "depth": 1, "3ddet": 1},
+                           img_size=(64, 128), patch=4, embed_dim=16, depths=(2, 2, 2, 2), heads=(1, 2, 4, 8), window=6,
+                           img_ds_ratio=1.0, level_embed_dim=12, f=24, chan_embed_dim=16, chan_nheads=4, head="deconv"),
+        # tps_mid with the 3ddet task: window 12, 0.75 input scaling, dd_label_map_size
+        "tps_mid3d": dict(tasks=["semseg", "depth", "3ddet"], num_output={"semseg": 19, "depth": 1, "3ddet": 1},
+                          img_size=(256, 512), patch=4, embed_dim=16, depths=(2, 2, 2, 2), heads=(1, 2, 4, 8), window=12,
+                          img_ds_ratio=0.75, level_embed_dim=16, f=24, chan_embed_dim=16, chan_nheads=1, head="deconv",
+                          dd_label_map_size=(128, 256)),
+        # the reference's Cityscapes-3D model exactly (cs_swinB_taskprompter.yml: semseg, depth, 3ddet)
+        "tps_swinB3d": dict(tasks=["semseg", "depth", "3ddet"], num_output={"semseg": 19, "depth": 1, "3ddet": 1},
+                            img_size=(1024, 2048), patch=4, embed_dim=128, depths=(2, 2, 18, 2), heads=(4, 8, 16, 32),
+                            window=12, img_ds_ratio=0.75, level_embed_dim=256, f=450, chan_embed_dim=256, chan_nheads=1,
+                            head="deconv", dd_label_map_size=(512, 1024)),
     }[name]
     c = dict(c)
     c["name"] = name

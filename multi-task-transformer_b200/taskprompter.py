@@ -382,7 +382,11 @@ class DEConvHead(_HeadForward, nn.Module):
 class TaskPrompterWrapper(nn.Module):
     """models/taskprompter_wrapper.py:9-40: backbone -> per-task head -> bilinear resize to the input size (or
     p.dd_label_map_size; the '3ddet' task is NOT resized, :34-38). forward(x [B,3,H,W]) -> {task: [B,n_out,H,W]}
-    fp32, written into the plan's static buffers (clone to keep results across calls)."""
+    fp32, written into the plan's static buffers (clone to keep results across calls).
+
+    With a TaskPrompterSwin backbone, heads['3ddet'] may be any nn.Module (in practice the reference's FCOS3DHead): it
+    runs in PyTorch on the 4 level maps the fused forward leaves in static buffers, on the same stream, and its output
+    is out['3ddet'] as the head returns it (the hybrid head, INTEGRATION.md section 1)."""
 
     def __init__(self, p, backbone, heads, nsplit=PARITY, use_graph=True):
         super().__init__()
@@ -393,30 +397,47 @@ class TaskPrompterWrapper(nn.Module):
         self.target_size = tuple(p.dd_label_map_size) if "dd_label_map_size" in keys else None
         self.nsplit = nsplit
         self.use_graph = use_graph
+        swin = self._swin()
         for t in self.tasks:
+            if swin and t == "3ddet":
+                if t not in heads or not isinstance(heads[t], nn.Module):
+                    raise ValueError("mtt_b200 TaskPrompterSwin: the '3ddet' task needs a detection head module in "
+                                     "heads['3ddet'] (the reference's FCOS3DHead, or any module taking the 4 level maps)")
+                continue
             if not isinstance(heads[t], (ConvHead, DEConvHead)):
                 raise NotImplementedError(f"mtt_b200: unsupported head {type(heads[t]).__name__} for task {t!r} (the "
                                           "FCOS3D detection head of the reference needs mmdet3d: SURVEY.md 8f N4)")
 
+    def _swin(self):
+        return type(self.backbone).__name__ == "TaskPrompterSwin"
+
     def plan(self, batch, device, postproc=False):
         mode = "postproc" if postproc else "full"
         P = _Plan
-        if type(self.backbone).__name__ == "TaskPrompterSwin":       # the Swin family has its own launch plan
+        if self._swin():                                              # the Swin family has its own launch plan
             from .taskprompter_swin import _SwinPlan as P
         return _plan_for(self, (int(batch), torch.device(device), int(self.nsplit), mode), lambda: P(
             self.backbone, self.heads, self.tasks, self.target_size, batch, torch.device(device), self.nsplit, mode=mode))
 
+    def _run(self, x, postproc):
+        out = self.plan(x.shape[0], x.device, postproc=postproc).run(x, graph=self.use_graph)
+        if self._swin() and "3ddet" in out:          # wrapper :37-38: the detection head on the level maps, not resized
+            with _dev_ctx(x.device):
+                out["3ddet"] = self.heads["3ddet"](out["3ddet"])
+        return out
+
     def forward(self, x):
         _check_input(self, x)
-        return self.plan(x.shape[0], x.device).run(x, graph=self.use_graph)
+        return self._run(x, postproc=False)
 
     def predict(self, x):
         """forward + the reference's `get_output` post-processing (TaskPrompter/utils/utils.py:27-63) fused
         into the final resize: {task: int64 [B,H,W] class map | fp32 map} without materialising the
         full-resolution logits (semseg / human_parts argmax, edge 255*sigmoid, sal 255*softmax[1], normals
-        (normalize+1)*255/2, depth clamp)."""
+        (normalize+1)*255/2, depth clamp). With a Swin backbone, '3ddet' holds the detection head's RAW output: the
+        reference's get_output('3ddet') decodes boxes with p.detmodel (mmdet3d), which this library does not have."""
         _check_input(self, x)
-        return self.plan(x.shape[0], x.device, postproc=True).run(x, graph=self.use_graph)
+        return self._run(x, postproc=True)
 
 
 # --------------------------------------------------------------------------------------------
@@ -638,6 +659,17 @@ def build_from_config(cfg, nsplit=PARITY, use_graph=True):
     return TaskPrompterWrapper(p, bb, heads, nsplit=nsplit, use_graph=use_graph)
 
 
+def _mirror_head(t, hd):
+    """This library's ConvHead (:688-698) or DEConvHead (:700-715) shaped like the reference head hd, told apart by the
+    first layer (parameters are loaded afterwards)."""
+    if not hasattr(hd, "mt_proj") or not hasattr(hd, "linear_pred"):
+        raise NotImplementedError(f"mtt_b200.accelerate: unsupported head {type(hd).__name__} for task {t!r} "
+                                  "(FCOS3DHead / '3ddet' needs mmdet3d: SURVEY.md 8f N4)")
+    if isinstance(hd.mt_proj[0], nn.ConvTranspose2d):
+        return DEConvHead(hd.mt_proj[0].weight.shape[0], hd.linear_pred.weight.shape[0])
+    return ConvHead(hd.linear_pred.weight.shape[1], hd.linear_pred.weight.shape[0])
+
+
 def accelerate(ref_model, nsplit=PARITY, use_graph=True):
     """Drop-in: build the fused wrapper from a REFERENCE TaskPrompterWrapper instance. Parameters and BatchNorm
     statistics are COPIED (`load_state_dict(ref.state_dict(), strict=True)`: same names, so the copy is exact);
@@ -652,15 +684,7 @@ def accelerate(ref_model, nsplit=PARITY, use_graph=True):
                            chan_nheads=bb.blocks[0].attn.chan_nheads,
                            drop_path_rate=float(getattr(bb.blocks[-1].drop_path, "drop_prob", 0.0) or 0.0))
 
-    def mirror(t, hd):   # ConvHead (:688-698) or DEConvHead (:700-715), told apart by the first layer
-        if not hasattr(hd, "mt_proj") or not hasattr(hd, "linear_pred"):
-            raise NotImplementedError(f"mtt_b200.accelerate: unsupported head {type(hd).__name__} for task {t!r} "
-                                      "(FCOS3DHead / '3ddet' needs mmdet3d: SURVEY.md 8f N4)")
-        if isinstance(hd.mt_proj[0], nn.ConvTranspose2d):
-            return DEConvHead(hd.mt_proj[0].weight.shape[0], hd.linear_pred.weight.shape[0])
-        return ConvHead(hd.linear_pred.weight.shape[1], hd.linear_pred.weight.shape[0])
-
-    heads = nn.ModuleDict({t: mirror(t, ref_model.heads[t]) for t in ref_model.tasks})
+    heads = nn.ModuleDict({t: _mirror_head(t, ref_model.heads[t]) for t in ref_model.tasks})
     m = TaskPrompterWrapper(p, mine_bb, heads, nsplit=nsplit, use_graph=use_graph)
     m.load_state_dict(ref_model.state_dict(), strict=True)
     return m.eval()

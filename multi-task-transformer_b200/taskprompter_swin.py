@@ -29,8 +29,13 @@ sequence, captured in a CUDA graph. What runs where:
 Exact algebraic re-orderings (results equal up to fp32 rounding): the bilinear x2 of the gated maps (TP:747-748) is applied
 AFTER the 1x1 decode convs and fea_fuse[0] instead of before -- bilinear resampling and per-pixel linear maps commute --
 which runs those convolutions at a quarter of the pixels.
-Unsupported (raises): the '3ddet' task (FCOS3D head, needs mmdet3d), absolute position embedding (ape=True; no reference
-config uses it). Eval mode only.
+The '3ddet' task of the reference's Cityscapes-3D config (semseg, depth, 3ddet) is an ordinary task in the backbone: its
+prompt row takes part in every window attention, channel attention and PatchMerging, and it has gating, decode convs and
+fea_fuse at each level. Its level features stay at the level's own resolution (no bilinear x2, TP:741, :764) and are not
+fused across scales (no multi_scale_fuse['3ddet'], TP:635, :709-710): the plan writes them as 4 NCHW maps
+[B, f, h_l, w_l], and TaskPrompterWrapper hands them to heads['3ddet'] -- the reference's FCOS3DHead (mmcv / mmdet3d), or any
+module -- which runs in PyTorch on the same stream. The library has no kernels for that head.
+Unsupported (raises): absolute position embedding (ape=True; no reference config uses it). Eval mode only.
 """
 import math
 from types import SimpleNamespace
@@ -39,11 +44,12 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .plans import Plan, _cached, _dev_ctx, _f32, _lin, _pack_stem, _predict_outputs
-from .taskprompter import (PARITY, Mlp, PatchEmbed, _HeadSpace, _launch_head, _pack_fuse, _pack_head,
+from .plans import Plan, _cached, _check_input, _dev_ctx, _f32, _lin, _pack_stem, _plan_for, _predict_outputs
+from .taskprompter import (PARITY, Mlp, PatchEmbed, _HeadSpace, _launch_head, _mirror_head, _pack_fuse, _pack_head,
                            _trunc_normal_)
 
 STRIDES = (8, 16, 32, 32)          # utils/common_config.py:37: level il lives at 1/STRIDES[il] of the image
+DET = "3ddet"                      # the detection task: level maps at their own resolution, no multi-scale fusion
 
 
 # --------------------------------------------------------------------------------------------
@@ -154,9 +160,6 @@ class TaskPrompterSwin(nn.Module):
         if isinstance(img_size, int):
             img_size = (img_size, img_size)
         tasks = list(p.TASKS.NAMES)
-        if "3ddet" in tasks:
-            raise NotImplementedError("mtt_b200 TaskPrompterSwin: the '3ddet' task needs the FCOS3D head (mmdet3d): "
-                                      "SURVEY.md 8f N4")
         self.p = p
         self.num_layers = len(depths)
         self.embed_dim, self.depths, self.heads, self.window_size = embed_dim, tuple(depths), tuple(num_heads), window_size
@@ -192,7 +195,8 @@ class TaskPrompterSwin(nn.Module):
                 nn.Conv2d(f, f, 3, padding=1)) for t in tasks}))
             self.fea_decode_spa.append(nn.ModuleDict({t: nn.Sequential(nn.Conv2d(cur, Lv, 1)) for t in tasks}))
             self.fea_decode_chan.append(nn.ModuleDict({t: nn.Sequential(nn.Conv2d(cur, Lv, 1)) for t in tasks}))
-        self.multi_scale_fuse = nn.ModuleDict({t: nn.Conv2d(f, f, 3, padding=1) for t in tasks})
+        # TP:635: no multi-scale fusion for '3ddet', whose head takes the 4 level maps as they are
+        self.multi_scale_fuse = nn.ModuleDict({t: nn.Conv2d(f, f, 3, padding=1) for t in tasks if t != DET})
         self.layers = nn.Sequential(*[
             BasicLayer(i == self.num_layers - 1, p, embed_dim * 2 ** i,
                        (self.patch_grid[0] // 2 ** i, self.patch_grid[1] // 2 ** i), depths[i], num_heads[i], window_size,
@@ -204,8 +208,18 @@ class TaskPrompterSwin(nn.Module):
                 if m.bias is not None:
                     nn.init.zeros_(m.bias)
 
+    nsplit = PARITY
+    use_graph = False
+
     def forward(self, x):
-        raise RuntimeError("TaskPrompterSwin runs fused inside TaskPrompterWrapper.forward; call the wrapper")
+        """TP:674-718: ({task: [B, final_embed_dim, 2 h0, 2 w0]} after the multi-scale fusion for the 2D tasks, for
+        '3ddet' the list of the 4 level maps [B, final_embed_dim, h_l, w_l]; info = {}). Outputs are fresh tensors."""
+        _check_input(self, x)
+        tasks = list(self.p.TASKS.NAMES)
+        pl = _plan_for(self, (x.shape[0], x.device, self.nsplit, "backbone"), lambda: _SwinPlan(
+            self, None, tasks, None, x.shape[0], x.device, self.nsplit, mode="backbone"))
+        out = pl.run(x, graph=self.use_graph)
+        return {t: [m.clone() for m in v] if t == DET else v.clone() for t, v in out.items()}, {}
 
 
 # --------------------------------------------------------------------------------------------
@@ -252,11 +266,12 @@ def _pack_merge(dsm, device, ns):
 
 
 def _pack_swin_decoder(bb, tasks, device, ns):
+    """levels[il][ti] for every task; msf[k] for the k-th 2D task (the tasks other than '3ddet')."""
     def build():
         W = SimpleNamespace()
         W.levels = [[_pack_fuse(bb, il, t, device, ns) for t in tasks] for il in range(bb.num_layers)]
         W.msf = [ops.pack_conv_weight(_f32(bb.multi_scale_fuse[t].weight, device), bb.multi_scale_fuse[t].bias, None, ns)
-                 for t in tasks]
+                 for t in tasks if t != DET]
         return W
     return _cached(bb, ("decoder", device, ns, tuple(tasks)), build)
 
@@ -275,17 +290,23 @@ def chan_kv_chunks(rows, ce, L):
 
 class _SwinPlan(Plan):
     """Geometry, workspace and launch sequence of one TaskPrompterSwin wrapper forward. mode: "full" = wrapper forward
-    (logits at the output size), "postproc" = predict() (get_output fused into the final resize, same launch count)."""
+    (logits at the output size), "postproc" = predict() (get_output fused into the final resize, same launch count),
+    "backbone" = TaskPrompterSwin.forward alone (the task features, NCHW). In every mode a '3ddet' task yields the list
+    of its 4 level maps [B, f, h_l, w_l] (NCHW fp32, static buffers): the wrapper hands them to the detection head."""
 
     def __init__(self, bb, heads, tasks, target, B, device, nsplit, mode="full"):
         super().__init__((bb, heads), B, device, nsplit, max(len(tasks), 2))
-        if mode not in ("full", "postproc"):
-            raise NotImplementedError(f"mtt_b200 TaskPrompterSwin: no {mode!r} plan (the wrapper forward and predict() "
-                                      "are built)")
+        if mode not in ("full", "postproc", "backbone"):
+            raise NotImplementedError(f"mtt_b200 TaskPrompterSwin: no {mode!r} plan (the wrapper forward, predict() "
+                                      "and the backbone forward are built)")
         device = self.dev
         self.bb, self.heads, self.tasks, self.target, self.mode = bb, heads, list(tasks), target, mode
         self.postproc = mode == "postproc"
         self.T = T = len(self.tasks)
+        self.det = self.tasks.index(DET) if DET in self.tasks else None
+        self.t2 = [t for t in self.tasks if t != DET]          # the 2D tasks: multi-scale fusion and a dense head
+        self.i2 = [self.tasks.index(t) for t in self.t2]       # ... and their rows among the T prompts
+        T2 = len(self.t2)
         p = bb.p
         self.ce = ce = p.chan_embed_dim
         self.r = int(round(math.sqrt(ce)))
@@ -358,22 +379,31 @@ class _SwinPlan(Plan):
                 d.ws_gate = ops.workspace(ops.workspace_bytes(ops.OP_GATED_CONV1X1, rows=B * d.P, Cdim=Cl, nsplit=ns, T=T),
                                           device)
                 d.cat = [S(B * d.P, 2 * self.Lv_pad, zero=True) for _ in range(T)]
-                d.g32 = [z(B * d.P, self.f_ld) for _ in range(T)]
-                d.up = [S(B * 4 * d.P, self.f, zero=True) for _ in range(T)]
-                d.mid = [S(B * 4 * d.P, self.f, zero=True) for _ in range(T)]
-                d.out32 = None if il == 0 else [z(B * 4 * d.P, self.f_ld) for _ in range(T)]
+                d.g32 = [z(B * d.P, self.f_ld) for _ in range(T2)]
+                d.up = [S(B * 4 * d.P, self.f, zero=True) for _ in range(T2)]
+                d.mid = [S(B * 4 * d.P, self.f, zero=True) for _ in range(T2)]
+                d.out32 = None if il == 0 else [z(B * 4 * d.P, self.f_ld) for _ in range(T2)]
+                if self.det is not None:         # fea_fuse of '3ddet' on the level's own map (TP:741, :764: no x2)
+                    d.det0, d.det1 = S(B * d.P, self.f, zero=True), S(B * d.P, self.f, zero=True)
+                    d.det32 = z(B * d.P, self.f_ld)
                 self.lv.append(d)
             h0, w0 = 2 * self.lv[0].h, 2 * self.lv[0].w
             self.fh, self.fw = h0, w0
-            self.acc = [z(B * h0 * w0, self.f_ld) for _ in range(T)]
-            self.accs = [S(B * h0 * w0, self.f, zero=True) for _ in range(T)]
-            self.hs = [_HeadSpace(hw, B, h0, w0, device, ns) for hw in self.Wh]
+            self.acc = [z(B * h0 * w0, self.f_ld) for _ in range(T2)]
+            self.accs = [S(B * h0 * w0, self.f, zero=True) for _ in range(T2)]
             oh, ow = self.target if self.target is not None else self.img
             self.out_hw = (oh, ow)
+            self.det_out = [z(B, self.f, d.h, d.w) for d in self.lv] if self.det is not None else None
+            if mode == "backbone":
+                self.hs = None
+                self.fea32 = [z(B * h0 * w0, self.f_ld) for _ in range(T2)]
+                self.out = {t: z(B, self.f, h0, w0) for t in self.t2}
+                return
+            self.hs = [_HeadSpace(hw, B, h0, w0, device, ns) for hw in self.Wh]
             if self.postproc:
-                self.out = _predict_outputs(self.tasks, B, (oh, ow), device)
+                self.out = _predict_outputs(self.t2, B, (oh, ow), device)
             else:
-                self.out = {t: z(B, hw.n_out, oh, ow) for t, hw in zip(self.tasks, self.Wh)}
+                self.out = {t: z(B, hw.n_out, oh, ow) for t, hw in zip(self.t2, self.Wh)}
 
     def _pack(self):
         bb, dev, ns = self.bb, self.dev, self.ns
@@ -381,7 +411,11 @@ class _SwinPlan(Plan):
         self.Wb = [[_pack_swin_block(blk, dev, ns) for blk in layer.blocks] for layer in bb.layers]
         self.Wm = [_pack_merge(layer.downsample, dev, ns) if layer.downsample is not None else None for layer in bb.layers]
         self.Wd = _pack_swin_decoder(bb, self.tasks, dev, ns)
-        self.Wh = [_pack_head(self.heads[t], dev, ns) for t in self.tasks]
+        # the 2D heads; the '3ddet' head (FCOS3D) is the caller's module and runs after the plan (TaskPrompterWrapper)
+        self.Wh = [_pack_head(self.heads[t], dev, ns) for t in self.t2] if self.mode != "backbone" else None
+
+    def _result(self):
+        return {t: list(self.det_out) if t == DET else self.out[t] for t in self.tasks}
 
     # ------------------------------------------------------------------------------------------
     def _block(self, s, w, blk):
@@ -439,26 +473,52 @@ class _SwinPlan(Plan):
                           [(tw.spa, tw.spa_b, tw.chan, tw.chan_b, d.cat[ti]) for ti, tw in enumerate(lvw)],
                           self.Lv, self.Lv_pad, d.ws_gate, B=B, T=T, N=T + d.P, H=d.heads, Cdim=d.C, gh=d.h, gw=d.w,
                           nh=self.nh, nw=self.nw)                                                   # :736-751 (1x1 first)
-        ops.gemm_grouped([(d.cat[ti], tw.f0, dict(bias=tw.f0_b, out_f32=d.g32[ti][:, :self.f], N=self.f))
-                          for ti, tw in enumerate(lvw)])                                           # fea_fuse[0]
-        self.streams.par([lambda ti=ti: ops.bilinear(d.g32[ti], self.f_ld, B, d.h, d.w, self.f, 2 * d.h, 2 * d.w,
-                                                     out_split=d.up[ti]) for ti in range(T)])     # :747-748 (moved)
-        ops.gemm_grouped([(d.up[ti], tw.f1, dict(N=self.f, K=self.f, bias=tw.f1_b, act=ops.ACT_GELU, out_split=d.mid[ti],
-                                                 conv=(B, 2 * d.h, 2 * d.w, 3, 1))) for ti, tw in enumerate(lvw)])
-        dst = self.acc if il == 0 else d.out32
-        ops.gemm_grouped([(d.mid[ti], tw.f4, dict(N=self.f, K=self.f, bias=tw.f4_b, out_f32=dst[ti][:, :self.f],
-                                                  conv=(B, 2 * d.h, 2 * d.w, 3, 1))) for ti, tw in enumerate(lvw)])
-        if il > 0:                                                                                  # TP:713-716
-            self.streams.par([lambda ti=ti: ops.bilinear(d.out32[ti], self.f_ld, B, 2 * d.h, 2 * d.w, self.f, self.fh,
-                                                         self.fw, out_f32=self.acc[ti][:, :self.f], accumulate=True)
-                              for ti in range(T)])
+        if self.t2:      # the 2D tasks; k indexes them, ti the task among all T
+            two = [(k, d.cat[ti], lvw[ti]) for k, ti in enumerate(self.i2)]
+            K2 = range(len(two))
+            ops.gemm_grouped([(cat, tw.f0, dict(bias=tw.f0_b, out_f32=d.g32[k][:, :self.f], N=self.f))
+                              for k, cat, tw in two])                                              # fea_fuse[0]
+            self.streams.par([lambda k=k: ops.bilinear(d.g32[k], self.f_ld, B, d.h, d.w, self.f, 2 * d.h, 2 * d.w,
+                                                       out_split=d.up[k]) for k in K2])            # :747-748 (moved)
+            ops.gemm_grouped([(d.up[k], tw.f1, dict(N=self.f, K=self.f, bias=tw.f1_b, act=ops.ACT_GELU,
+                                                    out_split=d.mid[k], conv=(B, 2 * d.h, 2 * d.w, 3, 1)))
+                              for k, _, tw in two])
+            dst = self.acc if il == 0 else d.out32
+            ops.gemm_grouped([(d.mid[k], tw.f4, dict(N=self.f, K=self.f, bias=tw.f4_b, out_f32=dst[k][:, :self.f],
+                                                     conv=(B, 2 * d.h, 2 * d.w, 3, 1))) for k, _, tw in two])
+            if il > 0:                                                                              # TP:713-716
+                self.streams.par([lambda k=k: ops.bilinear(d.out32[k], self.f_ld, B, 2 * d.h, 2 * d.w, self.f, self.fh,
+                                                           self.fw, out_f32=self.acc[k][:, :self.f], accumulate=True)
+                                  for k in K2])
+        if self.det is not None:
+            self._det_level(il)
+
+    def _det_level(self, il):
+        """fea_fuse of '3ddet' at level il on the level's own h x w map (TP:741, :764 skip the bilinear x2), written as
+        the NCHW level map the detection head takes (TP:709-710)."""
+        B, d, f = self.B, self.lv[il], self.f
+        tw = self.Wd.levels[il][self.det]
+        ops.gemm(d.cat[self.det], tw.f0, bias=tw.f0_b, out_split=d.det0, N=f)                     # fea_fuse[0]
+        ops.gemm(d.det0, tw.f1, N=f, K=f, bias=tw.f1_b, act=ops.ACT_GELU, out_split=d.det1,
+                 conv=(B, d.h, d.w, 3, 1))                                                          # fea_fuse[1..3]
+        ops.gemm(d.det1, tw.f4, N=f, K=f, bias=tw.f4_b, out_f32=d.det32[:, :f], conv=(B, d.h, d.w, 3, 1))   # [4]
+        ops.nhwc_to_nchw(d.det32, self.f_ld, B, f, d.h, d.w, self.det_out[il])
+
+    def _fused(self, k, out_split=None, out_f32=None):
+        """multi_scale_fuse of the k-th 2D task on the level sum (TP:711-717)."""
+        wm, bm = self.Wd.msf[k]
+        ops.split_f32(self.acc[k][:, :self.f], self.ns, out=self.accs[k])
+        ops.gemm(self.accs[k], wm, N=self.f, K=self.f, bias=bm, out_split=out_split, out_f32=out_f32,
+                 conv=(self.B, self.fh, self.fw, 3, 1))
+
+    def _fea_chain(self, k, t):
+        self._fused(k, out_f32=self.fea32[k][:, :self.f])
+        ops.nhwc_to_nchw(self.fea32[k], self.f_ld, self.B, self.f, self.fh, self.fw, self.out[t])
 
     def _head_chain(self, ti, t, hw, hs):
         B = self.B
         oh, ow = self.out_hw
-        wm, bm = self.Wd.msf[ti]
-        ops.split_f32(self.acc[ti][:, :self.f], self.ns, out=self.accs[ti])
-        ops.gemm(self.accs[ti], wm, N=self.f, K=self.f, bias=bm, out_split=hs.up, conv=(B, self.fh, self.fw, 3, 1))  # :717
+        self._fused(ti, out_split=hs.up)                                                            # :717
         _launch_head(hs, hw)
         if self.postproc:
             ops.bilinear_postproc(hs.pred, hs.pred.stride(0), B, hs.ph, hs.pw, hw.n_out, oh, ow,
@@ -489,12 +549,17 @@ class _SwinPlan(Plan):
         last = self.st[-1]
         ops.layernorm(last.x, W.nw, W.nb, W.neps, out_f32=self.xfin)                               # :709
         self._level(n_stage - 1, self.xfin, last.logits, last.rc)
+        if self.mode == "backbone":
+            self.streams.par([lambda k=k, t=t: self._fea_chain(k, t) for k, t in enumerate(self.t2)])
+            return
         self.streams.par([lambda ti=ti, t=t, hw=hw, hs=hs: self._head_chain(ti, t, hw, hs)
-                          for ti, (t, hw, hs) in enumerate(zip(self.tasks, self.Wh, self.hs))])
+                          for ti, (t, hw, hs) in enumerate(zip(self.t2, self.Wh, self.hs))])
 
 
-def build_from_config(cfg, nsplit=PARITY, use_graph=True):
-    """cfg: dict as in configs.taskprompter_swin() (mirrors TP/utils/common_config.py:34-41,64-90)."""
+def build_from_config(cfg, nsplit=PARITY, use_graph=True, det_head=None):
+    """cfg: dict as in configs.taskprompter_swin() (mirrors TP/utils/common_config.py:34-41,64-90). A config with the
+    '3ddet' task needs det_head: the nn.Module that takes the 4 level maps (the reference's FCOS3DHead,
+    utils/common_config.py:52-57, or any stand-in); it runs in PyTorch after the fused forward."""
     from .taskprompter import ConvHead, DEConvHead, TaskPrompterWrapper
     h, w = cfg["img_size"]
     E = cfg["embed_dim"]
@@ -509,5 +574,38 @@ def build_from_config(cfg, nsplit=PARITY, use_graph=True):
     bb = TaskPrompterSwin(p, img_size=(h, w), patch_size=cfg["patch"], embed_dim=E, depths=tuple(cfg["depths"]),
                           num_heads=tuple(cfg["heads"]), window_size=cfg["window"])
     head_cls = DEConvHead if cfg.get("head", "conv") == "deconv" else ConvHead
-    heads = nn.ModuleDict({t: head_cls(cfg["f"], cfg["num_output"][t]) for t in cfg["tasks"]})
+    if DET in cfg["tasks"] and det_head is None:
+        raise ValueError("TaskPrompterSwin: the '3ddet' task needs det_head= (the module that takes the 4 level maps, "
+                         "e.g. the reference's FCOS3DHead)")
+    heads = nn.ModuleDict({t: det_head if t == DET else head_cls(cfg["f"], cfg["num_output"][t]) for t in cfg["tasks"]})
     return TaskPrompterWrapper(p, bb, heads, nsplit=nsplit, use_graph=use_graph)
+
+
+def accelerate(ref_model, nsplit=PARITY, use_graph=True):
+    """Drop-in for a REFERENCE TaskPrompterWrapper around TaskPrompterSwin (two- or three-task). The geometry is read
+    from the instance; the backbone and the 2D heads are COPIED (`load_state_dict(ref.state_dict(), strict=True)`), so a
+    later in-place update of `ref_model` is not seen -- call `load_state_dict` again. The '3ddet' head (FCOS3DHead) is
+    the reference's module itself, SHARED: the library has no kernels for it, it runs in PyTorch on the 4 level maps."""
+    from .taskprompter import TaskPrompterWrapper
+    bb = ref_model.backbone
+    p = bb.p
+    if getattr(bb, "ape", False):
+        raise NotImplementedError("mtt_b200 TaskPrompterSwin: absolute position embedding is not supported")
+    ratio = p.img_ds_ratio
+    img = (p.ori_spatial_dim[0][0] * STRIDES[0], p.ori_spatial_dim[0][1] * STRIDES[0])       # common_config.py:37-39
+    if [int(s * ratio) for s in img] != list(bb.patch_embed.img_size):
+        raise ValueError(f"accelerate: cannot recover the input size from ori_spatial_dim {p.ori_spatial_dim} and the "
+                         f"patch embedding's {tuple(bb.patch_embed.img_size)} at ratio {ratio}")
+    blk0 = bb.layers[0].blocks[0]
+    mine_bb = TaskPrompterSwin(p, img_size=img, patch_size=bb.patch_embed.patch_size[0],
+                               in_chans=bb.patch_embed.proj.in_channels, embed_dim=bb.embed_dim,
+                               depths=tuple(len(layer.blocks) for layer in bb.layers),
+                               num_heads=tuple(layer.blocks[0].num_heads for layer in bb.layers),
+                               # stage 0 has the largest map: its window is the configured one unless every stage clips
+                               window_size=blk0.window_size, mlp_ratio=bb.mlp_ratio,
+                               qkv_bias=blk0.attn.qkv.bias is not None)
+    heads = nn.ModuleDict({t: ref_model.heads[t] if t == DET else _mirror_head(t, ref_model.heads[t])
+                           for t in ref_model.tasks})
+    m = TaskPrompterWrapper(p, mine_bb, heads, nsplit=nsplit, use_graph=use_graph)
+    m.load_state_dict(ref_model.state_dict(), strict=True)
+    return m.eval()
