@@ -49,9 +49,9 @@ def f32(x):
     return float(torch.tensor(x, dtype=torch.float32))
 
 
-def nan_split(ops, rows, cols, dev, extra_ld=8):
-    """A NaN-filled Split with one trailing row and extra_ld pad columns past round_up(cols, 8)."""
-    sp = ops.Split(rows + 1, cols, dev, ld=ops.round_up(cols, 8) + extra_ld)
+def nan_split(ops, rows, cols, dev, extra_ld=8, ns=2):
+    """A NaN-filled Split of ns planes with one trailing row and extra_ld pad columns past round_up(cols, 8)."""
+    sp = ops.Split(rows + 1, cols, dev, ns, ld=ops.round_up(cols, 8) + extra_ld)
     sp.buf.fill_(NAN)
     return sp
 
@@ -67,17 +67,32 @@ def pad_cols(v):
     return torch.as_strided(v, (v.shape[0], v.stride(0) - v.shape[1]), (v.stride(0), 1), v.storage_offset() + v.shape[1])
 
 
-def split_in(ops, x, pad=8):
-    """x fp32 [rows, cols] -> Split with NaN pad columns (what the kernel reads) and its float64 decoding."""
+def split_in(ops, x, pad=8, ns=2):
+    """x fp32 [rows, cols] -> Split of ns planes with NaN pad columns (what the kernel reads) and its float64 decoding."""
     rows, cols = x.shape
-    sp = ops.Split(rows, cols, x.device, ld=ops.round_up(cols, 8) + pad)
+    sp = ops.Split(rows, cols, x.device, ns, ld=ops.round_up(cols, 8) + pad)
     sp.buf.fill_(NAN)
-    ops.split_f32(x, out=sp)
+    ops.split_f32(x, ns, out=sp)
     return sp, decode(sp, rows, cols)
 
 
 def decode(sp, rows, cols):
-    return sp.buf[0, :rows, :cols].double() + sp.buf[1, :rows, :cols].double()
+    """float64 value of the planes: hi + lo, or hi alone."""
+    v = sp.buf[0, :rows, :cols].double()
+    return v + sp.buf[1, :rows, :cols].double() if sp.nsplit == 2 else v
+
+
+def split_rel(ns):
+    """Relative error of storing a value as ns planes (asserted as 2^-16 for hi + lo, 2^-8 for hi alone)."""
+    return 2.0 ** -16 if ns == 2 else 2.0 ** -8
+
+
+def assert_split_of(sp, x, what):
+    """The planes are the split of fp32 x bit for bit (hi alone when there is one plane)."""
+    rows, cols = x.shape
+    hi, lo = split_exact(x)
+    assert torch.equal(sp.buf[0, :rows, :cols], hi), f"{what}: hi plane"
+    assert sp.nsplit == 1 or torch.equal(sp.buf[1, :rows, :cols], lo), f"{what}: lo plane"
 
 
 def split_exact(x):
@@ -110,9 +125,10 @@ def assert_bounded(got, ref, bound, block, what):
 # ---------------------------------------------------------------------------------------------------------------------
 # window attention
 # ---------------------------------------------------------------------------------------------------------------------
-def _attention_case(ops, dev, *, B, nWy, nWx, ws, shift, T, heads, dh, seed):
+def _attention_case(ops, dev, *, B, nWy, nWx, ws, shift, T, heads, dh, seed, ns=2):
     """B images of nWy x nWx windows; q of every other query row scaled 12x so that its logits span about +-50 (the
-    online softmax rescales many times); bias table at std 0.5; shift mask (-100) when shift > 0."""
+    online softmax rescales many times); bias table at std 0.5; shift mask (-100) when shift > 0. qkv and the output
+    as ns planes. Returns the worst err / bound ratios of the output and the raw logits."""
     g = torch.Generator(device=dev).manual_seed(seed)
     C, L = heads * dh, ws * ws
     N, nW = T + L, nWy * nWx
@@ -120,13 +136,13 @@ def _attention_case(ops, dev, *, B, nWy, nWx, ws, shift, T, heads, dh, seed):
     x = torch.randn(rows, 3 * C, device=dev, generator=g)
     qs = torch.where(torch.arange(rows, device=dev) % N % 2 == 0, 12.0, 1.0)
     x[:, :C] *= qs[:, None]
-    qkv, X = split_in(ops, x)
+    qkv, X = split_in(ops, x, ns=ns)
     table = torch.randn((2 * ws - 1) ** 2, heads, device=dev, generator=g) * 0.5
     bias = table[R.relative_position_index(ws).reshape(-1).to(dev)].reshape(L, L, heads).permute(2, 0, 1)  # [h, q, k]
     biasT = bias.transpose(1, 2).contiguous()                                                 # the kernel's [h, key, query]
     mask = R.shifted_window_mask(nWy * ws, nWx * ws, ws, shift).to(dev) if shift else None    # [nW, q, k]
     maskT = mask.transpose(1, 2).contiguous() if shift else None
-    out = nan_split(ops, rows, C, dev)
+    out = nan_split(ops, rows, C, dev, ns=ns)
     raw_buf = torch.full((BW * heads * T * L + 16,), NAN, device=dev)
     raw = raw_buf[:BW * heads * T * L].view(BW, heads, T, L)
     scale = f32(dh ** -0.5)
@@ -147,13 +163,17 @@ def _attention_case(ops, dev, *, B, nWy, nWx, ws, shift, T, heads, dh, seed):
     # exp(2 d) - 1 ~ 2 d, times |v_j - o| <= 2 max|v|; the fp32 accumulation of N weighted v rows and 1/l; split 2^-16.
     d = U * (dh + 4) * As.amax(-1, keepdim=True) + 2.0 ** -21
     vmax = v.abs().amax((-1, -2), keepdim=True)
-    bound = (4 * d + (N + 3) * U) * vmax + 2.0 ** -16 * o.abs()
+    bound = (4 * d + (N + 3) * U) * vmax + split_rel(ns) * o.abs()
     got = decode(out, rows, C).view(BW, N, heads, dh).transpose(1, 2)
-    assert_bounded(got, o, bound, 2, f"attention out (B={B} nW={nW} ws={ws} shift={shift} T={T} dh={dh})")
+    assert_bounded(got, o, bound, 2, f"attention out (B={B} nW={nW} ws={ws} shift={shift} T={T} dh={dh} ns={ns})")
     assert_untouched(out, rows, C)
+    ratios = [float(((got - o).abs() / bound).max())]
     if T:
-        assert_bounded(raw.double(), dot[..., :T, T:], U * (dh + 1) * A[..., :T, T:], 2, "raw prompt logits")
+        rb = U * (dh + 1) * A[..., :T, T:]
+        assert_bounded(raw.double(), dot[..., :T, T:], rb, 2, "raw prompt logits")
+        ratios.append(float(((raw.double() - dot[..., :T, T:]).abs() / rb).max()))
     assert torch.isnan(raw_buf[raw.numel():]).all() and (T or torch.isnan(raw_buf).all()), "raw written past its end"
+    return ratios
 
 
 @pytest.mark.parametrize("stage", range(4))
@@ -231,7 +251,13 @@ def _unwindow(w, ws, shift, B, H, W):
     (2, 25, 49, 97, 3, 3, 0),
 ])
 def test_window_gather_scatter(ops, cuda_dev, B, H, W, C, T, heads, shift):
-    ws, dev = 12, cuda_dev
+    _gather_scatter_case(ops, cuda_dev, B=B, H=H, W=W, C=C, T=T, heads=heads, ws=12, shift=shift)
+
+
+def _gather_scatter_case(ops, dev, *, B, H, W, C, T, heads, ws, shift, ns=2, lasts=(False, True)):
+    """Window gather into ns planes (bit-exact), and the scatter with last = each of `lasts`: xa and x += xa bit-exact,
+    the logits map [B, heads, T, T + H*W] bit-exact with its T prefix columns untouched, the prompt mean within its
+    bound. Returns the prompt mean's worst err / bound."""
     g = torch.Generator(device=dev).manual_seed(H * W + C + shift)
     rnd = lambda *s: torch.randn(*s, device=dev, generator=g)
     Hp, Wp = -(-H // ws) * ws, -(-W // ws) * ws
@@ -241,14 +267,14 @@ def test_window_gather_scatter(ops, cuda_dev, B, H, W, C, T, heads, shift):
     xn, pn = padded(B * H * W, C, dev), padded(B * T, C, dev)
     xn.copy_(rnd(B * H * W, C))
     pn.copy_(rnd(B * T, C))
-    sw = nan_split(ops, rows, C, dev)
+    sw = nan_split(ops, rows, C, dev, ns=ns)
     ops.swin_window_gather(xn, pn, sw, B=B, H=H, W=W, Cdim=C, T=T, ws=ws, shift=shift)
     torch.cuda.synchronize()
     win = _windows(xn.reshape(B, H, W, C), ws, shift)
     pr = pn.reshape(B, 1, T, C).expand(B, nW, T, C).reshape(B * nW, T, C)
-    hi, lo = split_exact(torch.cat([pr, win], 1).reshape(rows, C))            # the T prompts first in every window
-    assert torch.equal(sw.buf[0, :rows, :C], hi) and torch.equal(sw.buf[1, :rows, :C], lo)
+    assert_split_of(sw, torch.cat([pr, win], 1).reshape(rows, C), "window gather")   # the T prompts first in every window
     assert_untouched(sw, rows, C)
+    del sw, win, pr
 
     # scatter: xa = window reverse (copy), x += xa (torch's fp32 add), p += window mean of the prompt rows, logits map
     o = padded(rows, C, dev)
@@ -260,7 +286,8 @@ def test_window_gather_scatter(ops, cuda_dev, B, H, W, C, T, heads, shift):
     lg_ref = lg_ref.reshape(B, H * W, heads, T).permute(0, 2, 3, 1)
     pm = ow[:, :T].double().reshape(B, nW, T, C)
     x0, p0 = rnd(B * H * W, C), rnd(B * T, C)
-    for last in (False, True):
+    ratio = 0.0
+    for last in lasts:
         xa, x, p = padded(B * H * W, C, dev), padded(B * H * W, C, dev, fill=7.0), padded(B * T, C, dev, fill=7.0)
         x.copy_(x0)
         p.copy_(p0)
@@ -280,6 +307,8 @@ def test_window_gather_scatter(ops, cuda_dev, B, H, W, C, T, heads, shift):
             want = p0.double() + pm.mean(1).reshape(B * T, C)
             bound = U * ((-(-nW // 4) + 4) * pm.abs().mean(1).reshape(B * T, C) + p0.double().abs() + want.abs())
             assert_bounded(p.double(), want, bound, 1, "prompt mean")
+            ratio = max(ratio, float(((p.double() - want).abs() / bound).max()))
+    return ratio
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -332,7 +361,13 @@ def test_chan_kv_splitk_swinB(ops, cuda_dev, stage):
     (2, 3, 1003, 4),                                                     # 4 x 4 windows of 4 x 4; C % 8 != 0
 ])
 def test_chan_attention(ops, cuda_dev, B, T, C, nh):
-    ce, dev = 256, cuda_dev
+    _chan_attention_case(ops, cuda_dev, B=B, T=T, C=C, nh=nh)
+
+
+def _chan_attention_case(ops, dev, *, B, T, C, nh, ns=2):
+    """swin_chan_attention at ce = 256 with nh x nh channel windows, the split output as ns planes: raw_chan and
+    chan_out within their bounds, the split bit-exact. Returns the worst err / bound of raw_chan and chan_out."""
+    ce = 256
     r = 16
     wh = ww = r // nh
     G, we = nh * nh, wh * ww
@@ -343,7 +378,7 @@ def test_chan_attention(ops, cuda_dev, B, T, C, nh):
     kv = padded(B * C, 2 * ce, dev)
     kv.copy_(torch.randn(B * C, 2 * ce, device=dev, generator=gen))
     co = padded(B * T, ce, dev)
-    cs = nan_split(ops, B * T, ce, dev)
+    cs = nan_split(ops, B * T, ce, dev, ns=ns)
     rc_buf = torch.full((B * T * C * G + 16,), NAN, device=dev)
     rc = rc_buf[:B * T * C * G].view(B, T, C, nh, nh)
     ops.swin_chan_attention(q, kv, co, cs, rc, B=B, T=T, Cdim=C, ce=ce, nh=nh, nw=nh)
@@ -366,12 +401,13 @@ def test_chan_attention(ops, cuda_dev, B, T, C, nh):
     vmax = vg.abs().amax((-1, -2), keepdim=True)
     bound = (4 * d + (C // 8 + 12) * U) * vmax
     got_rc = rc.double().permute(0, 3, 4, 1, 2).reshape(B, G, T, C)
+    got_co = grid(co.double().reshape(B, T, ce))
     assert_bounded(got_rc, raw, rb, 3, "raw_chan")
-    assert_bounded(grid(co.double().reshape(B, T, ce)), out, bound, 3, "chan_out")
+    assert_bounded(got_co, out, bound, 3, "chan_out")
     assert torch.isnan(pad_cols(co)).all() and torch.isnan(rc_buf[rc.numel():]).all()
-    hi, lo = split_exact(co.contiguous())                                    # the split output is the split of chan_out
-    assert torch.equal(cs.buf[0, :B * T, :ce], hi) and torch.equal(cs.buf[1, :B * T, :ce], lo)
+    assert_split_of(cs, co.contiguous(), "chan_out split")                  # the split output is the split of chan_out
     assert_untouched(cs, B * T, ce)
+    return [float(((got_rc - raw).abs() / rb).max()), float(((got_co - out).abs() / bound).max())]
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -398,9 +434,14 @@ def test_conv3x3_s2_maps(ops, cuda_dev, stage):
     """spa_attn_ds (TP:458-460) at the three Swin-B merges: Cin = Cout = heads * T = 8 / 16 / 32 over the full-size
     logit maps stored behind T prompt columns; columns before out_offset stay untouched."""
     H, W, _, heads = SWINB[stage]
-    B, T, dev = 1, 2, cuda_dev
-    Cin, L = heads * T, H * W
-    g = torch.Generator(device=dev).manual_seed(stage)
+    _conv3x3_s2_case(ops, cuda_dev, B=1, T=2, H=H, W=W, Cin=heads * 2, seed=stage)
+
+
+def _conv3x3_s2_case(ops, dev, *, B, T, H, W, Cin, seed):
+    """conv3x3_s2_maps over [B, Cin, T + H*W] logit maps (the T prompt columns first) into [B, Cin, T + H*W/4]:
+    within 9 Cin + 2 FMAs of the absolute conv, the T prefix columns untouched. Returns the worst err / bound."""
+    L = H * W
+    g = torch.Generator(device=dev).manual_seed(seed)
     x = torch.randn(B, Cin, T + L, device=dev, generator=g)
     w = torch.randn(Cin, Cin, 3, 3, device=dev, generator=g) * 0.2
     b = torch.randn(Cin, device=dev, generator=g)
@@ -412,15 +453,23 @@ def test_conv3x3_s2_maps(ops, cuda_dev, stage):
     want = F.conv2d(xm, w.double(), b.double(), stride=2, padding=1)
     absum = F.conv2d(xm.abs(), w.double().abs(), b.double().abs(), stride=2, padding=1)
     got = out[..., T:].double().reshape(want.shape)
-    assert_bounded(got, want, U * (9 * Cin + 2) * absum, 2, "conv3x3_s2")   # 9 Cin FMAs after the bias
+    bound = U * (9 * Cin + 2) * absum
+    assert_bounded(got, want, bound, 2, f"conv3x3_s2 B={B} Cin={Cin} {H}x{W}")   # 9 Cin FMAs after the bias
     assert torch.isnan(out[..., :T]).all()
+    return float(((got - want).abs() / bound).max())
 
 
 @pytest.mark.parametrize("nwin", [1, 4])
 def test_chan_up(ops, cuda_dev, nwin):
     """process_chan_attn (TP:463-466) at the last merge: C 1024 -> 2048 over the channel axis of raw_chan."""
-    BT, C, Cout, dev = 2, 1024, 2048, cuda_dev
-    g = torch.Generator(device=dev).manual_seed(nwin)
+    _chan_up_case(ops, cuda_dev, BT=2, C=1024, nwin=nwin, seed=nwin)
+
+
+def _chan_up_case(ops, dev, *, BT, C, nwin, seed):
+    """swin_chan_up C -> 2C over the channel axis of raw_chan [BT, C, nwin]; nothing past the output written. Returns
+    the worst err / bound."""
+    Cout = 2 * C
+    g = torch.Generator(device=dev).manual_seed(seed)
     rc = torch.randn(BT, C, nwin, device=dev, generator=g)
     w = torch.randn(Cout, C, device=dev, generator=g) * 0.05
     buf = torch.full((BT * Cout * nwin + 16,), NAN, device=dev)
@@ -428,5 +477,7 @@ def test_chan_up(ops, cuda_dev, nwin):
     ops.swin_chan_up(rc, w, out, BT=BT, Cdim=C, nwin=nwin)
     torch.cuda.synchronize()
     want = w.double() @ rc.double()
-    assert_bounded(out.double(), want, U * (C + 1) * (w.double().abs() @ rc.double().abs()), 1, "chan_up")
+    bound = U * (C + 1) * (w.double().abs() @ rc.double().abs())
+    assert_bounded(out.double(), want, bound, 1, f"chan_up BT={BT} C={C}")
     assert torch.isnan(buf[out.numel():]).all()
+    return float(((out.double() - want).abs() / bound).max())

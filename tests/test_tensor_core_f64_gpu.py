@@ -2,7 +2,8 @@
 against float64, element by element.
 
 Recording. A module fixture builds each benched plan (tp_cfg4, tp_cfg2, tp_cfg5, ip_cfg3, tps_swinB at
-bench.DEFAULT_BATCH, nsplit = 2, no graph) and runs one eager forward; tp_cfg4 and tp_cfg2 also run one eager
+bench.DEFAULT_BATCH, nsplit = 2, no graph) and the three-task tps_swinB3d (batch 1, nn.Identity as the 3ddet head: its
+window GEMMs have M = nW (3 + 144) rows) and runs one eager forward; tp_cfg4 and tp_cfg2 also run one eager
 TrainStep._fwd_bwd with the bench's criterion and labels. Pass-through recorders around ops.gemm, gemm_grouped,
 gemm_splitk, attention and the five composites of csrc/block_ops.cu turn every call into a geometry key (call_key): the
 shapes, the mode, the epilogue (act, bias, residual kind), the row maps (regroup, a_gather), the offsets, which outputs
@@ -105,7 +106,8 @@ TEETH_FRAC = 0.10
 TAIL_STAGES = 32          # keys with at most this many K-stages must show the ragged-tail defect (see the docstring)
 F32_SENT = 0x7FC0BEEF     # one fixed NaN payload, so that an untouched element keeps its exact bits
 BF16_SENT = 0x7FA5        # the pattern test_tc_exact_gpu._sentinel_split writes
-FORWARD = ["tp_cfg4", "tp_cfg2", "tp_cfg5", "ip_cfg3", "tps_swinB"]
+FORWARD = ["tp_cfg4", "tp_cfg2", "tp_cfg5", "ip_cfg3", "tps_swinB", "tps_swinB3d"]
+EXTRA_BATCH = {"tps_swinB3d": 1}   # forwards the bench does not run: their batch
 TRAIN = ["tp_cfg4", "tp_cfg2"]
 RECORDED = ["gemm", "gemm_grouped", "gemm_splitk", "attention", "ln_qkv", "proj_residual", "ln_mlp_residual",
             "gated_conv1x1", "conv3x3_bn_act"]
@@ -963,8 +965,10 @@ def _build(name, dev, nsplit):
     import bench
     cfg, M, _ = bench.family(name)
     torch.manual_seed(0)
+    # a '3ddet' model takes its detection head from the caller; the plan ends at the 4 level maps it hands over
+    det = dict(det_head=torch.nn.Identity()) if "3ddet" in cfg["tasks"] and name.startswith("tps_") else {}
     with torch.device(dev):
-        return cfg, M.build_from_config(cfg, nsplit=nsplit, use_graph=False)
+        return cfg, M.build_from_config(cfg, nsplit=nsplit, use_graph=False, **det)
 
 
 def _record_run(ops, fn):
@@ -984,7 +988,7 @@ def _forward(name, dev, nsplit):
     ops = _ops()
     cfg, model = _build(name, dev, nsplit)
     model.eval()
-    x = torch.randn(bench.DEFAULT_BATCH[name], 3, *cfg["img_size"], device=dev)
+    x = torch.randn(EXTRA_BATCH.get(name) or bench.DEFAULT_BATCH[name], 3, *cfg["img_size"], device=dev)
     out = _record_run(ops, lambda: model(x))
     del model
     torch.cuda.empty_cache()
