@@ -206,7 +206,8 @@ def test_gate_split_at_the_3ddet_levels_f64(cuda_dev, ns):
     Swin level map (groups of P rows, no prompt rows), against float64 (2u per gated value + the split bound)."""
     import mtt_b200  # noqa: F401
     from mtt_b200 import ops
-    from test_forward_kernels_f64_gpu import Guarded, U, check_planes, gen, randn, ref_gates, round_up
+    from f64_checks import Guarded, U, check_planes, gen, randn, round_up
+    from kernel_cases import ref_gates
 
     cfg, levels = _levels()
     T, B = len(cfg["tasks"]), 1
@@ -244,8 +245,7 @@ def test_fea_fuse_convs_at_the_3ddet_levels_f64(cuda_dev, il):
     dropped lo x lo products, the fp32 accumulation over K = 9 * 450), GELU's slope (< 1.13) on top for fea_fuse[1..3]."""
     import mtt_b200  # noqa: F401
     from mtt_b200 import ops
-    from test_forward_kernels_f64_gpu import SPLIT, U, check, check_planes, gen, planes_value, randn
-    from test_train_kernels_f64_gpu import LAM
+    from f64_checks import LAM, SPLIT, U, check, check_planes, decode, gen, randn
 
     cfg, levels = _levels()
     (h, w), _, _ = levels[il]
@@ -255,7 +255,7 @@ def test_fea_fuse_convs_at_the_3ddet_levels_f64(cuda_dev, il):
     x = randn(g, B * h * w, f)
     a = ops.Split(B * h * w, f, "cuda", 2, zero=True)
     ops.split_f32(x, 2, out=a)
-    av = planes_value(a).view(B, h, w, f).permute(0, 3, 1, 2)
+    av = decode(a).view(B, h, w, f).permute(0, 3, 1, 2)
     wt = randn(g, f, f, 3, 3, scale=1 / math.sqrt(K))
     bias = randn(g, f, scale=0.1)
     bn = nn.BatchNorm2d(f).to("cuda").eval()

@@ -11,84 +11,45 @@ build records the same keys. The CPU variant does the same on tps_tiny3d and tps
 
 Float64. Every table entry runs on random inputs inside NaN sentinels (pad columns, guard rows, the T prompt columns of
 the logit maps, spare planes) that must come back bit-identical, in parity mode and, where the kernel writes split
-planes, in speed mode. Bounds and references are those of test_forward_kernels_f64_gpu.py (LayerNorm, gating,
-bilinear, post-processing) and test_swin_kernels_gpu.py (window attention, gather / scatter, channel attention,
-stride-2 convolution, channel up-projection); data movement is bit-exact. The input downsample 1024x2048 -> 768x1536 has
+planes, in speed mode. Bounds and references are those of tests/kernel_cases.py (LayerNorm, gating, bilinear,
+post-processing, window attention, gather / scatter, channel attention, stride-2 convolution, channel up-projection)
+under the error model of tests/f64_checks.py; data movement is bit-exact. The input downsample 1024x2048 -> 768x1536 has
 a fp32 scale of 4/3 that is not exact: ref_bilinear_any interpolates at the kernel's own coordinates and bounds their
 rounding. Beside the table: the stage-0 window scatter at B = 2 and conv3x3_s2_maps at B = 10, whose grid-stride loops
 only run past the 4096- / 8192-block caps of their launches. Every test prints its worst err / bound."""
-import inspect
-import math
-import sys
+import collections
 
 import pytest
 import torch
 import torch.nn as nn
 
-import test_forward_kernels_f64_gpu as F64
-import test_swin_kernels_gpu as SW
+from f64_checks import (Guarded, assert_planes_bit_exact, gen, guarded_split, ops, padded, randn,  # noqa: F401
+                        report, round_up)
+from kernel_cases import (E_BIL, attention_case, bilinear_case, chan_attention_case, chan_up_case, conv3x3_s2_case,
+                          fp32_coords_exact, gate_case, gather_scatter_case, layernorm_case, nan_split,
+                          assert_untouched, postproc_case, ref_bilinear, ref_bilinear_any, ref_im2col, rows_of)
 from oracle import configs
-from test_forward_kernels_f64_gpu import (Guarded, _bil, _frozen, assert_planes_bit_exact, gen, guarded_split,
-                                          randn, report, round_up)
+from plan_calls import DET, SwinGeom, bil, frozen, glue_key, recording
 
 pytestmark = [pytest.mark.timeout(1200)]      # the GPU tests are marked one by one: the CPU checks are not
 CONFIGS = ["tps_swinB", "tps_swinB3d"]
 MODES = ["full", "postproc", "backbone"]
-DET = "3ddet"
 RECORDED = ["layernorm", "split_f32", "im2col_patch", "broadcast_rows", "swin_window_gather", "swin_window_attention",
             "swin_window_scatter", "transpose_split", "swin_chan_attention", "swin_merge_gather", "conv3x3_s2_maps",
             "swin_chan_up", "gated_conv1x1", "bilinear", "bilinear_postproc", "nhwc_to_nchw"]
-STRIDES = (8, 16, 32, 32)           # decoder level il at 1 / STRIDES[il] of the full image (before img_ds_ratio)
 
 
 # ---- geometry ------------------------------------------------------------------------------------------------------------
-class SwinGeom:
-    """One Swin TaskPrompter forward at batch B, from its config: stages, decoder levels, head and output sizes."""
-
-    def __init__(self, name, B=1):
-        cfg = configs.taskprompter_swin(name)
-        self.name, self.cfg, self.B = name, cfg, B
-        self.tasks = list(cfg["tasks"])
-        self.T = len(self.tasks)
-        self.t2 = [t for t in self.tasks if t != DET]
-        self.img = tuple(cfg["img_size"])
-        r = cfg["img_ds_ratio"]
-        self.ds = tuple(int(s * r) for s in self.img)
-        self.patch, E = cfg["patch"], cfg["embed_dim"]
-        self.E = E
-        gh, gw = self.ds[0] // self.patch, self.ds[1] // self.patch
-        self.ce, self.nh = cfg["chan_embed_dim"], int(round(math.sqrt(cfg["chan_nheads"])))
-        self.stages = []
-        for i, (depth, heads) in enumerate(zip(cfg["depths"], cfg["heads"])):
-            H, W = gh >> i, gw >> i
-            ws, shift = cfg["window"], cfg["window"] // 2
-            if min(H, W) <= ws:                               # the window clipped to the map, no shift
-                ws, shift = min(H, W), 0
-            Hp, Wp = -(-H // ws) * ws, -(-W // ws) * ws
-            self.stages.append(dict(H=H, W=W, L=H * W, C=E << i, heads=heads, ws=ws, nW=(Hp // ws) * (Wp // ws),
-                                    shifts=[0 if j % 2 == 0 else shift for j in range(depth)], depth=depth))
-        self.f, self.Lv = cfg["f"], cfg["level_embed_dim"]
-        self.f_ld = round_up(self.f, 8)
-        chans = [2 * E, 4 * E, 8 * E, 8 * E]
-        self.levels = [dict(h=int(self.img[0] // s * r), w=int(self.img[1] // s * r), C=chans[il],
-                            heads=self.stages[il]["heads"]) for il, s in enumerate(STRIDES)]
-        self.fh, self.fw = 2 * self.levels[0]["h"], 2 * self.levels[0]["w"]
-        k = 2 if cfg.get("head", "conv") == "deconv" else 1
-        self.ph, self.pw = k * self.fh, k * self.fw            # the head's prediction map
-        self.out_hw = tuple(cfg.get("dd_label_map_size", self.img))
-        self.n_out = dict(cfg["num_output"])
-
-
 def swin_table(g, mode):
     """{function: [shape dicts]} of every recorded call one `mode` pass makes (duplicates kept out)."""
     from mtt_b200 import ops
     B, T, ce, nh = g.B, g.T, g.ce, g.nh
-    t = {fn: [] for fn in RECORDED}
+    t = collections.defaultdict(list)
     add = lambda fn, **d: None if d in t[fn] else t[fn].append(d)
     ln = lambda rows, cols, split=False: add("layernorm", rows=rows, cols=cols, ld_in=cols, f32=not split, split=split)
     sp32 = lambda rows, cols, ld_in: add("split_f32", rows=rows, cols=cols, ld_in=ld_in, ld_out=round_up(cols, 8))
     if g.ds != g.img:                                          # TP:676-677: every input channel as a 1-channel NCHW map
-        add("bilinear", **_bil(1, B * 3, *g.img, 1, *g.ds, "nchw"))
+        add("bilinear", **bil(1, B * 3, *g.img, 1, *g.ds, "nchw"))
     P0 = g.stages[0]["L"]
     add("im2col_patch", shape=(B, 3) + g.ds, patch=g.patch, ld=round_up(3 * g.patch ** 2, 8))
     ln(B * P0, g.E)
@@ -119,12 +80,12 @@ def swin_table(g, mode):
             ln(B * L, C)                                       # the final norm (TP:709)
     for il, lv in enumerate(g.levels):                         # cal_task_feature (TP:721-774)
         h, w, C, P = lv["h"], lv["w"], lv["C"], lv["h"] * lv["w"]
-        add("gated_conv1x1", B=B, T=T, N=T + P, H=lv["heads"], C=C, gh=h, gw=w, nh=nh, nw=nh, x_group_rows=P,
+        add("gate_split", B=B, T=T, N=T + P, H=lv["heads"], C=C, gh=h, gw=w, nh=nh, nw=nh, x_group_rows=P,
             x_row_offset=0, ldx=C, ntasks=T)
         if g.t2:
-            add("bilinear", **_bil(g.f_ld, B, h, w, g.f, 2 * h, 2 * w, "split", ld_out=g.f_ld))
+            add("bilinear", **bil(g.f_ld, B, h, w, g.f, 2 * h, 2 * w, "split", ld_out=g.f_ld))
             if il > 0:
-                add("bilinear", **_bil(g.f_ld, B, 2 * h, 2 * w, g.f, g.fh, g.fw, "f32", ld_out=g.f_ld, acc=True))
+                add("bilinear", **bil(g.f_ld, B, 2 * h, 2 * w, g.f, g.fh, g.fw, "f32", ld_out=g.f_ld, acc=True))
         if DET in g.tasks:
             add("nhwc_to_nchw", ld_in=g.f_ld, B=B, Cd=g.f, H=h, W=w)
     for task in g.t2:                                          # multi_scale_fuse, then the head or the NCHW features
@@ -133,7 +94,7 @@ def swin_table(g, mode):
         if mode == "backbone":
             add("nhwc_to_nchw", ld_in=g.f_ld, B=B, Cd=g.f, H=g.fh, W=g.fw)
         elif mode == "full":
-            add("bilinear", **_bil(round_up(n, 4), B, g.ph, g.pw, n, *g.out_hw, "nchw"))
+            add("bilinear", **bil(round_up(n, 4), B, g.ph, g.pw, n, *g.out_hw, "nchw"))
         else:
             add("bilinear_postproc", ld_in=round_up(n, 4), B=B, h=g.ph, w=g.pw, C=n, H2=g.out_hw[0], W2=g.out_hw[1],
                 kind=ops.POSTPROC_KIND[task])
@@ -172,57 +133,6 @@ def entries(fn, split=True):
 
 
 # ---- recorded keys -----------------------------------------------------------------------------------------------------------
-def _key_of_call(fn, a):
-    """The table entry of one ops.<fn> call, a = its bound arguments; the shared glue through the forward file's."""
-    if fn == "gated_conv1x1":
-        return fn, dict(F64._key_of_call(fn, a)[1])
-    if fn in ("layernorm", "im2col_patch", "broadcast_rows", "bilinear", "bilinear_postproc", "nhwc_to_nchw"):
-        return F64._key_of_call(fn, a)
-    if fn == "split_f32":
-        x, o = a["x"], a["out"]
-        assert a["cols_pad"] in (None, x.shape[1])
-        return fn, dict(rows=x.shape[0], cols=x.shape[1], ld_in=x.stride(0), ld_out=o.ld)
-    if fn in ("swin_window_gather", "swin_window_scatter"):
-        d = dict(B=a["B"], H=a["H"], W=a["W"], C=a["Cdim"], T=a["T"], ws=a["ws"], shift=a["shift"])
-        if fn == "swin_window_gather":
-            return fn, dict(d, ldx=a["xn"].stride(0), ldp=a["pn"].stride(0), ld_out=a["out"].ld)
-        return fn, dict(d, heads=a["heads"], last=bool(a["last"]), ldo=a["o32"].stride(0), ldxa=a["xa"].stride(0),
-                        ldx=a["x"].stride(0), ldp=a["p"].stride(0))
-    if fn == "swin_window_attention":
-        return fn, dict(BW=a["BW"], nW=a["nW"], T=a["T"], L=a["L"], heads=a["heads"], C=a["out"].cols,
-                        scale=a["scale"], masked=a["maskT"] is not None, ldq=a["qkv"].ld, ldo=a["out"].ld)
-    if fn == "transpose_split":
-        return fn, dict(B=a["B"], L=a["L"], C=a["Cdim"], ld_in=a["x"].stride(0), ld_out=a["out"].ld)
-    if fn == "swin_chan_attention":
-        return fn, dict(B=a["B"], T=a["T"], C=a["Cdim"], ce=a["ce"], nh=a["nh"], nw=a["nw"], ldq=a["q"].stride(0),
-                        ldkv=a["kv"].stride(0), ldco=a["co32"].stride(0), ldcs=a["cos"].ld)
-    if fn == "swin_merge_gather":
-        return fn, dict(B=a["B"], H=a["H"], W=a["W"], C=a["Cdim"], ldx=a["x"].stride(0), ldo=a["out"].stride(0))
-    if fn == "conv3x3_s2_maps":
-        return fn, dict(B=a["B"], Cin=a["Cin"], Cout=a["w"].shape[0], H=a["H"], W=a["W"], in_stride=a["in_stride"],
-                        in_offset=a["in_offset"], out_stride=a["out_stride"], out_offset=a["out_offset"])
-    if fn == "swin_chan_up":
-        return fn, dict(BT=a["BT"], C=a["Cdim"], Cout=a["w"].shape[0], nwin=a["nwin"])
-    raise KeyError(fn)
-
-
-def install_recorders(monkeypatch, seen):
-    """Pass-through recorders around ops.<RECORDED>. Only calls made from the library's own modules are recorded (an
-    emulated composite calling another emulated function is not a plan call)."""
-    from mtt_b200 import ops
-    for fn in RECORDED:
-        orig = getattr(ops, fn)
-        sig = inspect.signature(orig)
-
-        def rec(*a, _fn=fn, _orig=orig, _sig=sig, **k):
-            if sys._getframe(1).f_globals.get("__name__", "").startswith("mtt_b200"):
-                ba = _sig.bind(*a, **k)
-                ba.apply_defaults()
-                seen.append(_key_of_call(_fn, ba.arguments))
-            return _orig(*a, **k)
-        monkeypatch.setattr(ops, fn, rec)
-
-
 def build(name, dev, nsplit):
     from mtt_b200 import taskprompter_swin as TS
     cfg = configs.taskprompter_swin(name)
@@ -241,18 +151,21 @@ def run_mode(model, mode, x):
         return model.backbone(x)
 
 
-def recorded_keys(model, mode, x, seen):
-    """The distinct keys of one pass of `mode` (after an unrecorded pass that builds the plan and packs the weights)."""
+def recorded_keys(model, mode, x):
+    """The distinct keys of one pass of `mode` (after an unrecorded pass that builds the plan and packs the weights).
+    Only calls from the library's modules are recorded: an emulated composite calling another emulated function is not
+    a plan call."""
+    from mtt_b200 import ops
     run_mode(model, mode, x)
-    seen.clear()
-    run_mode(model, mode, x)
-    if x.is_cuda:
-        torch.cuda.synchronize()
-    return {(fn, _frozen(d)) for fn, d in seen}
+    with recording(ops, RECORDED, glue_key, [], library_only=True) as seen:
+        run_mode(model, mode, x)
+        if x.is_cuda:
+            torch.cuda.synchronize()
+    return {(fn, frozen(d)) for fn, d in seen}
 
 
 def tabled_keys(g, mode):
-    return {(fn, _frozen(d)) for fn, ds in swin_table(g, mode).items() for d in ds}
+    return {(fn, frozen(d)) for fn, ds in swin_table(g, mode).items() for d in ds}
 
 
 def assert_same_keys(got, want, what):
@@ -264,24 +177,22 @@ def assert_same_keys(got, want, what):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", CONFIGS)
-def test_plans_call_exactly_the_tabled_shapes(cuda_dev, monkeypatch, name):
+def test_plans_call_exactly_the_tabled_shapes(cuda_dev, name):
     """One eager pass of each mode at batch 1, parity build: recorded keys == table; a speed-mode build of the wrapper
     forward records the same keys (the keys hold no plane count)."""
     import mtt_b200  # noqa: F401
     g = geom(name)
-    seen = []
-    install_recorders(monkeypatch, seen)
     x = torch.randn(g.B, 3, *g.img, device=cuda_dev)
     model = build(name, cuda_dev, 2)
     for mode in MODES:
-        got = recorded_keys(model, mode, x, seen)
+        got = recorded_keys(model, mode, x)
         assert_same_keys(got, tabled_keys(g, mode), f"{name} {mode}")
         print(f"{name} {mode}: {len(got)} distinct calls, exactly the table's")
-    par = recorded_keys(model, "full", x, seen)
+    par = recorded_keys(model, "full", x)
     del model
     torch.cuda.empty_cache()
     model = build(name, cuda_dev, 1)
-    assert recorded_keys(model, "full", x, seen) == par, f"{name}: the speed-mode plan calls other shapes"
+    assert recorded_keys(model, "full", x) == par, f"{name}: the speed-mode plan calls other shapes"
     del model
     torch.cuda.empty_cache()
 
@@ -297,12 +208,10 @@ def test_plans_call_exactly_the_tabled_shapes_emulated(monkeypatch, name):
     monkeypatch.setattr(TP, "_check_input", lambda mod, x: None)
     monkeypatch.setattr(TS, "_check_input", lambda mod, x: None)
     g = SwinGeom(name, B=2)
-    seen = []
-    install_recorders(monkeypatch, seen)
     x = torch.randn(g.B, 3, *g.img)
     model = build(name, "cpu", 2)
     for mode in MODES:
-        assert_same_keys(recorded_keys(model, mode, x, seen), tabled_keys(g, mode), f"{name} {mode}")
+        assert_same_keys(recorded_keys(model, mode, x), tabled_keys(g, mode), f"{name} {mode}")
 
 
 def test_geometry_of_the_swinB_models():
@@ -313,20 +222,13 @@ def test_geometry_of_the_swinB_models():
         assert {d["L"] for d in tab["swin_window_attention"]} == {144}
         assert {d["Cin"] for d in tab["conv3x3_s2_maps"]} == {4 * T, 8 * T, 16 * T}
         assert {"rows": 73728, "cols": 128, "ld_in": 128, "f32": True, "split": False} in tab["layernorm"]
-        assert _bil(1, 3, 1024, 2048, 1, 768, 1536, "nchw") in tab["bilinear"]
+        assert bil(1, 3, 1024, 2048, 1, 768, 1536, "nchw") in tab["bilinear"]
         assert {(d["h"], d["w"], d["H2"], d["W2"]) for d in tab["bilinear_postproc"]} == {(384, 768, 512, 1024)}
     assert len(table("tps_swinB3d")["nhwc_to_nchw"]) == 3 + 1          # 3 distinct level maps (two share 24x48) + fea
-    assert not F64.fp32_coords_exact(1024, 768) and F64.fp32_coords_exact(384, 512)
+    assert not fp32_coords_exact(1024, 768) and fp32_coords_exact(384, 512)
 
 
 # ---- float64: window attention, gather / scatter, channel attention, merging ------------------------------------------------
-@pytest.fixture(scope="module")
-def ops(cuda_dev):
-    import mtt_b200  # noqa: F401
-    from mtt_b200 import ops as o
-    return o
-
-
 def _stage_of(g, C):
     return next(s for s in g.stages if s["C"] == C)
 
@@ -338,7 +240,7 @@ def test_window_attention(ops, cuda_dev, name, i, ns):
     d = table(name)["swin_window_attention"][i]
     s = _stage_of(geom(name), d["C"])
     shift = 6 if d["masked"] else 0
-    r = SW._attention_case(ops, cuda_dev, B=d["BW"] // d["nW"], nWy=s["H"] // s["ws"], nWx=s["W"] // s["ws"],
+    r = attention_case(ops, cuda_dev, B=d["BW"] // d["nW"], nWy=s["H"] // s["ws"], nWx=s["W"] // s["ws"],
                            ws=s["ws"], shift=shift, T=d["T"], heads=d["heads"], dh=d["C"] // d["heads"],
                            seed=100 * i + d["T"], ns=ns)
     report(f"window attention {name} C={d['C']} shift={shift} ns={ns} (out, raw logits)", r)
@@ -346,7 +248,7 @@ def test_window_attention(ops, cuda_dev, name, i, ns):
 
 
 def _gather_scatter(ops, dev, d, ns, B=None):
-    r = SW._gather_scatter_case(ops, dev, B=B or d["B"], H=d["H"], W=d["W"], C=d["C"], T=d["T"], heads=d["heads"],
+    r = gather_scatter_case(ops, dev, B=B or d["B"], H=d["H"], W=d["W"], C=d["C"], T=d["T"], heads=d["heads"],
                                 ws=d["ws"], shift=d["shift"], ns=ns, lasts=(d["last"],))
     torch.cuda.empty_cache()
     return r
@@ -378,13 +280,13 @@ def test_transpose_split(ops, cuda_dev, name, i, ns):
     """[B, L, C] -> split [B*C, L] per stage (L = 73728 ... 1152), NaN pad columns read past C would show: bit-exact."""
     d = table(name)["transpose_split"][i]
     B, L, C = d["B"], d["L"], d["C"]
-    x = SW.padded(B * L, C, cuda_dev)
+    x = padded(B * L, C, cuda_dev)
     x.copy_(randn(gen(200 + i), B * L, C))
-    out = SW.nan_split(ops, B * C, L, cuda_dev, ns=ns)
+    out = nan_split(B * C, L, cuda_dev, ns=ns)
     ops.transpose_split(x, out, B=B, L=L, Cdim=C)
     torch.cuda.synchronize()
-    SW.assert_split_of(out, x.reshape(B, L, C).transpose(1, 2).reshape(B * C, L), "transpose_split")
-    SW.assert_untouched(out, B * C, L)
+    assert_planes_bit_exact(out, x.reshape(B, L, C).transpose(1, 2).reshape(B * C, L), "transpose_split")
+    assert_untouched(out, B * C, L)
 
 
 @pytest.mark.gpu
@@ -392,7 +294,7 @@ def test_transpose_split(ops, cuda_dev, name, i, ns):
 def test_chan_attention(ops, cuda_dev, name, i, ns):
     """Channel attention of the T prompts over the C channels of each stage (C = 128 ... 1024, one 16 x 16 window)."""
     d = table(name)["swin_chan_attention"][i]
-    r = SW._chan_attention_case(ops, cuda_dev, B=d["B"], T=d["T"], C=d["C"], nh=d["nh"], ns=ns)
+    r = chan_attention_case(ops, cuda_dev, B=d["B"], T=d["T"], C=d["C"], nh=d["nh"], ns=ns)
     report(f"chan attention {name} T={d['T']} C={d['C']} ns={ns} (raw_chan, chan_out)", r)
 
 
@@ -402,7 +304,7 @@ def test_merge_gather(ops, cuda_dev, name, i, ns):
     """2 x 2 merge (0,0), (1,0), (0,1), (1,1) at each merging stage: bit-exact, pad columns untouched."""
     d = table(name)["swin_merge_gather"][i]
     B, H, W, C = d["B"], d["H"], d["W"], d["C"]
-    x = SW.padded(B * H * W, C, cuda_dev)
+    x = padded(B * H * W, C, cuda_dev)
     x.copy_(randn(gen(300 + i), B * H * W, C))
     gb = Guarded((B * H * W // 4, d["ldo"] + 4), torch.float32)
     gb.snapshot()
@@ -419,7 +321,7 @@ def test_conv3x3_s2_maps(ops, cuda_dev, name, i, ns):
     """spa_attn_ds at each merge: Cin = Cout = heads * T (8 / 16 / 32 at T = 2, 12 / 24 / 48 at T = 3)."""
     d = table(name)["conv3x3_s2_maps"][i]
     T = d["in_offset"]
-    r = SW._conv3x3_s2_case(ops, cuda_dev, B=d["B"], T=T, H=d["H"], W=d["W"], Cin=d["Cin"], seed=400 + i)
+    r = conv3x3_s2_case(ops, cuda_dev, B=d["B"], T=T, H=d["H"], W=d["W"], Cin=d["Cin"], seed=400 + i)
     report(f"conv3x3_s2 {name} Cin={d['Cin']}", [r])
 
 
@@ -428,7 +330,7 @@ def test_conv3x3_s2_maps_grid_stride(ops, cuda_dev):
     """Stage 0 at B = 10, Cin = 12: 10 * 12 * 96 * 192 = 2 211 840 outputs > 8192 blocks of 256: the loop runs."""
     d = table("tps_swinB3d")["conv3x3_s2_maps"][0]
     assert d["Cin"] == 12 and 10 * 12 * (d["H"] // 2) * (d["W"] // 2) > 8192 * 256
-    report("conv3x3_s2 B=10 Cin=12", [SW._conv3x3_s2_case(ops, cuda_dev, B=10, T=3, H=d["H"], W=d["W"], Cin=12,
+    report("conv3x3_s2 B=10 Cin=12", [conv3x3_s2_case(ops, cuda_dev, B=10, T=3, H=d["H"], W=d["W"], Cin=12,
                                                           seed=499)])
 
 
@@ -437,7 +339,7 @@ def test_conv3x3_s2_maps_grid_stride(ops, cuda_dev):
 def test_chan_up(ops, cuda_dev, name, i, ns):
     """process_chan_attn C -> 2C at each merge, B * T rows."""
     d = table(name)["swin_chan_up"][i]
-    r = SW._chan_up_case(ops, cuda_dev, BT=d["BT"], C=d["C"], nwin=d["nwin"], seed=500 + i)
+    r = chan_up_case(ops, cuda_dev, BT=d["BT"], C=d["C"], nwin=d["nwin"], seed=500 + i)
     report(f"chan_up {name} BT={d['BT']} C={d['C']}", [r])
 
 
@@ -453,7 +355,7 @@ def test_im2col_patch(ops, name, i, ns):
     gb.snapshot()
     ops.im2col_patch(img, d["patch"], sp)
     gb.unchanged_outside(reg, "im2col_patch")
-    assert_planes_bit_exact(sp, F64.ref_im2col(img, d["patch"]), "im2col_patch")
+    assert_planes_bit_exact(sp, ref_im2col(img, d["patch"]), "im2col_patch")
 
 
 @pytest.mark.gpu
@@ -465,7 +367,7 @@ def test_broadcast_rows(ops, name, i, ns):
     gb = Guarded((d["B"] * d["group_rows"], d["ld"]), torch.float32)
     gb.snapshot()
     ops.broadcast_rows(src, gb.view, d["B"], d["group_rows"])
-    rows = F64.rows_of(d["B"], d["T"], d["group_rows"], 0, "cuda")
+    rows = rows_of(d["B"], d["T"], d["group_rows"], 0, "cuda")
     gb.unchanged_outside((rows, slice(0, d["C"])), "broadcast_rows")
     assert torch.equal(gb.view[rows, :d["C"]], src.repeat(d["B"], 1))
 
@@ -491,16 +393,16 @@ def test_layernorm(ops, name, i, ns):
     split planes (4C = 512 ... 4096 columns), the final norm."""
     d = table(name)["layernorm"][i]
     report(f"layernorm {name} {d['rows']}x{d['cols']} split={d['split']} ns={ns}",
-           [F64.layernorm_case(ops, d, 700 + i, ns)])
+           [layernorm_case(ops, d, 700 + i, ns)])
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("gated_conv1x1"))
+@pytest.mark.parametrize("name,i,ns", entries("gate_split"))
 def test_gate(ops, name, i, ns):
     """The gating stage of gated_conv1x1 at each decoder level: all T tasks in one launch, x = the level map (group
     P, offset 0), prompt logits [B, heads, T, T + P], channel logits of the 2C up-projection."""
-    d = table(name)["gated_conv1x1"][i]
-    report(f"gate {name} level C={d['C']} {d['gh']}x{d['gw']} ns={ns}", F64.gate_case(ops, d, ns, name, seed=800 + i))
+    d = table(name)["gate_split"][i]
+    report(f"gate {name} level C={d['C']} {d['gh']}x{d['gw']} ns={ns}", gate_case(ops, d, ns, name, seed=800 + i))
 
 
 @pytest.mark.gpu
@@ -511,7 +413,7 @@ def test_bilinear(ops, name, i, ns):
     384x768 -> 512x1024 (scale 0.75, exact)."""
     d = table(name)["bilinear"][i]
     report(f"bilinear {name} {d['h']}x{d['w']}->{d['H2']}x{d['W2']} {d['form']} ns={ns}",
-           [F64.bilinear_case(ops, d, ns, 900 + i)])
+           [bilinear_case(ops, d, ns, 900 + i)])
     torch.cuda.empty_cache()
 
 
@@ -521,7 +423,7 @@ def test_bilinear_postproc(ops, name, i, ns):
     """predict()'s final resize fused with get_output: semseg argmax over 19 classes exact where the float64 top-2
     margin exceeds twice the logit bound, depth (kind 4) within the logit bound."""
     d = table(name)["bilinear_postproc"][i]
-    r = F64.postproc_case(ops, d, 950 + i)
+    r = postproc_case(ops, d, 950 + i)
     if r is not None:
         report(f"bilinear_postproc {name} kind {d['kind']}", [r])
 
@@ -576,8 +478,8 @@ def test_bilinear_any_ratio_reference():
     for (h, w, H2, W2) in ((12, 16, 9, 12), (7, 11, 10, 13), (30, 40, 23, 31), (9, 12, 12, 16)):
         x = torch.randn(B * h * w, C) * 3
         rows = torch.arange(B * h * w)
-        y, a, ec = F64.ref_bilinear_any(x.double(), rows, B, h, w, C, H2, W2)
-        bound = F64.E_BIL * a + ec
+        y, a, ec = ref_bilinear_any(x.double(), rows, B, h, w, C, H2, W2)
+        bound = E_BIL * a + ec
         for fma in (False, True):
             got = _kernel_bilinear_cpu(x, B, h, w, C, H2, W2, fma).double()
             assert bool(((got - y).abs() <= bound).all()), (h, w, H2, W2, fma, float(((got - y).abs() / bound).max()))
@@ -586,8 +488,8 @@ def test_bilinear_any_ratio_reference():
             o = torch.zeros(B, C, H2, W2)
             ops.bilinear(x, C, B, h, w, C, H2, W2, out_nchw=o)
         assert bool(((o.double() - y).abs() <= bound).all()), (h, w, H2, W2, "emul_ops")
-        if F64.fp32_coords_exact(h, H2) and F64.fp32_coords_exact(w, W2):
-            y2, a2 = F64.ref_bilinear(x.double(), rows, B, h, w, C, H2, W2)
+        if fp32_coords_exact(h, H2) and fp32_coords_exact(w, W2):
+            y2, a2 = ref_bilinear(x.double(), rows, B, h, w, C, H2, W2)
             torch.testing.assert_close(y, y2, rtol=1e-13, atol=1e-13)
         bad = _kernel_bilinear_cpu(x, B, h, w, C, H2, W2, False, coord=lambda sc, d: sc * (d - 0.5)).double()
         assert bool(((bad - y).abs() > bound).any()), (h, w, H2, W2, "a shifted coordinate is not caught")

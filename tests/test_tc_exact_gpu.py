@@ -12,8 +12,8 @@ Every case keeps sum|terms| <= 2^22 per output element (asserted from the genera
 hold integers of the same size as hi, so that the three issued products are told apart, and a swapped plane or an
 extra lo*lo product changes the result.
 
-Outputs are compared as raw bits over the WHOLE buffer: every byte the kernel must not write keeps its sentinel (NaN
-or a bf16 pattern), so a stray store or a store to the wrong row fails too. The float64 references are written in plain
+Outputs are compared as raw bits over the WHOLE buffer: every byte the kernel must not write keeps its sentinel
+(tests/f64_checks.py), so a stray store or a store to the wrong row fails too. The float64 references are written in plain
 torch on the host (im2col + matmul for the convolutions); test_reference_builder_matches_emulation checks them against
 tests/emul_ops.py without a GPU.
 """
@@ -23,175 +23,18 @@ import math
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
-BOUND = 2 ** 22
+from f64_checks import assert_bits_equal, mtt_ops, sentinel, sentinel_split
+from kernel_cases import (BOUND, conv_case, conv_weight, gather_case, int_range, int_split, ints, plain_case,
+                          ref_gemm, regroup_case, to_dev)
+
 LN2 = float(np.float32(math.log(2.0)))   # scale * log2(e) == 1 in fp32: the kernel's exp2 argument is exact
-
-
-def _ops():
-    import mtt_b200  # noqa: F401
-    from mtt_b200 import ops
-
-    return ops
-
-
-# ------------------------------------------------------------------------------------------------------------------
-# operands: integer planes written straight into Split.buf (split_f32 would give lo = 0 for small integers)
-# ------------------------------------------------------------------------------------------------------------------
-def _ints(g, shape, r):
-    return torch.randint(-r, r + 1, shape, generator=g).float()
-
-
-def _range(k_eff):
-    """Largest value range r (|hi|, |lo| <= r) that keeps sum|terms| of a k_eff-deep product well below BOUND."""
-    return max(1, min(16, math.isqrt(2 ** 19 // k_eff)))
-
-
-def _split(dev, g, rows, cols, r, nsplit=2, ld=None, pad=0.0, lo_zero=False):
-    """Split [rows, cols] with integer planes in [-r, r]; columns [cols, ld) hold `pad` (NaN: a poisoned pad)."""
-    ops = _ops()
-    sp = ops.Split(rows, cols, "cpu", nsplit, ld=ld)
-    sp.buf.fill_(pad)
-    sp.buf[0, :, :cols] = _ints(g, (rows, cols), r).bfloat16()
-    if nsplit == 2:
-        sp.buf[1, :, :cols] = 0 if lo_zero else _ints(g, (rows, cols), r).bfloat16()
-    return _to(sp, dev)
-
-
-def _to(sp, dev):
-    return _ops().Split.from_planes(sp.buf.to(dev, copy=True), sp.cols)
-
-
-def _conv_weight(dev, g, Cout, Cin, ks, r, nsplit=2):
-    """Packed conv weight [Cout, ks*ks*cin_pad] with integer hi and lo planes: pack_conv_weight of an integer hi tensor
-    and of an integer lo tensor, the second's hi plane copied into the first's lo plane (pad columns stay zero)."""
-    ops = _ops()
-    wh = _ints(g, (Cout, Cin, ks, ks), r)
-    wl = _ints(g, (Cout, Cin, ks, ks), r) if nsplit == 2 else None
-    if dev == "cpu":    # the host copy for the reference: the packed layout written out in torch
-        cp = (Cin + 63) // 64 * 64
-        sp = ops.Split(Cout, ks * ks * cp, "cpu", nsplit, zero=True)
-        for i, t in enumerate((wh, wl)[:nsplit]):
-            sp.buf[i].view(Cout, ks * ks, cp)[:, :, :Cin] = t.permute(0, 2, 3, 1).reshape(Cout, ks * ks, Cin).bfloat16()
-        return sp
-    hi, _ = ops.pack_conv_weight(wh.to(dev), None, None, nsplit)
-    if nsplit == 2:
-        lo, _ = ops.pack_conv_weight(wl.to(dev), None, None, 2)
-        hi.buf[1] = lo.buf[0]
-    return hi
-
-
-def _sentinel_f32(dev, rows, cols):
-    return torch.full((rows, cols), float("nan"), device=dev)
-
-
-def _sentinel_split(dev, rows, cols, nsplit=2, ld=None):
-    """A Split whose every element is a bf16 bit pattern no kernel store produces here (a NaN payload)."""
-    ops = _ops()
-    sp = ops.Split(rows, cols, dev, nsplit, ld=ld)
-    sp.buf.view(torch.int16).fill_(0x7fa5)
-    return sp
-
-
-# ------------------------------------------------------------------------------------------------------------------
-# the float64 reference of ops.gemm(): same arguments, writes the expected values into the given output buffers
-# ------------------------------------------------------------------------------------------------------------------
-def _planes(sp, nsplit):
-    hi = sp.buf[0].double()
-    return hi, (sp.buf[1].double() if nsplit == 2 else None)
-
-
-def _out_rows(r, regroup):
-    if regroup is None or regroup[0] == 0:
-        return r
-    stride = regroup[3] if len(regroup) > 3 else 1
-    return (r // regroup[0]) * regroup[1] + regroup[2] + (r % regroup[0]) * stride
-
-
-def _im2col(x, B, H, W, ks, dil):
-    """NHWC [B*H*W, K] -> [B*H*W, ks*ks*K], tap-major (the packed weight's column order), zero padding."""
-    K = x.shape[1]
-    p = dil * (ks // 2)
-    xp = F.pad(x.reshape(B, H, W, K), (0, 0, p, p, p, p))
-    cols = [xp[:, ky * dil:ky * dil + H, kx * dil:kx * dil + W, :] for ky in range(ks) for kx in range(ks)]
-    return torch.stack(cols, 3).reshape(B * H * W, ks * ks * K)
-
-
-def ref_gemm(a, w, *, M=None, N=None, K=None, bias=None, act=0, residual=None, res_row_mod=0, out_f32=None,
-             out_split=None, out_col_offset=0, regroup=None, conv=None, a_row_offset=0, a_gather=None, w_col_offset=0,
-             a_col_offset=0, w_row_offset=0, out_row_offset=0, sk_ws=None):
-    """Exact float64 restatement of ops.gemm on host tensors (a, w: Splits; outputs updated in place). Asserts the
-    sum|terms| bound that makes the kernel's fp32 arithmetic exact."""
-    nsplit = min(a.nsplit, w.nsplit)
-    M = a.rows if M is None else M
-    N = w.rows if N is None else N
-    K = a.cols if K is None else K
-    r = torch.arange(M)
-    if a_gather is not None:
-        arow = a_row_offset + (r // a_gather[0]) * a_gather[1] + r % a_gather[0]
-    else:
-        arow = a_row_offset + r
-    A = [None if p is None else p[arow][:, a_col_offset:a_col_offset + K] for p in _planes(a, nsplit)]
-    if conv is None:
-        Wp = [None if p is None else p[w_row_offset:w_row_offset + N, w_col_offset:w_col_offset + K]
-              for p in _planes(w, nsplit)]
-    else:
-        B, H, Wd, ks, dil = conv
-        cp = (K + 63) // 64 * 64
-        A = [None if p is None else _im2col(p, B, H, Wd, ks, dil) for p in A]
-        Wp = [None if p is None else p[w_row_offset:w_row_offset + N, :ks * ks * cp].reshape(N, ks * ks, cp)[:, :, :K]
-              .reshape(N, ks * ks * K) for p in _planes(w, nsplit)]
-    (ah, al), (wh, wl) = A, Wp
-    y = ah @ wh.t()
-    if nsplit == 2:
-        y = y + ah @ wl.t() + al @ wh.t()
-    # sum|terms| <= (largest row sum of |a_hi| + |a_lo|) * (largest |w_hi| + |w_lo|) + |bias| + |residual|
-    amag = ah.abs() + (al.abs() if nsplit == 2 else 0)
-    wmag = wh.abs() + (wl.abs() if nsplit == 2 else 0)
-    mag = float(amag.sum(1).max()) * float(wmag.max()) if M and N else 0.0
-    ro = _out_rows(r, regroup)
-    if bias is not None:
-        b = bias[:N].double().cpu()
-        y, mag = y + b, mag + float(b.abs().max())
-    if act == 2:
-        y = y.clamp_min(0)
-    else:
-        assert act == 0, "integer cases: no activation or ReLU"
-    if residual is not None:
-        rr = r % res_row_mod if res_row_mod > 0 else ro
-        res = residual.cpu()[rr, :N].double()
-        y, mag = y + res, mag + float(res.abs().max())
-    assert not torch.isnan(y).any() and mag <= BOUND, f"case out of the exact range: {mag}"
-    y32 = y.float()
-    if out_f32 is not None:
-        out_f32[ro, :N] = y32.to(out_f32.device)
-    if out_split is not None:
-        hi = y32.bfloat16()
-        rows, cols = ro + out_row_offset, slice(out_col_offset, out_col_offset + N)
-        out_split.buf[0, rows.to(out_split.buf.device), cols] = hi.to(out_split.buf.device)
-        if out_split.nsplit == 2:
-            out_split.buf[1, rows.to(out_split.buf.device), cols] = (y32 - hi.float()).bfloat16().to(out_split.buf.device)
-
-
-def _bits(t):
-    t = t.detach().cpu().contiguous()
-    return t.view(torch.int32) if t.dtype == torch.float32 else t.view(torch.int16)
-
-
-def _assert_bits_equal(got, want, what):
-    g, w = _bits(got), _bits(want)
-    if not torch.equal(g, w):
-        bad = (g != w).nonzero()
-        i = tuple(bad[0].tolist())
-        raise AssertionError(f"{what}: {bad.shape[0]} of {g.numel()} elements differ, first at {i}: "
-                             f"got {got.cpu()[i].item()}, want {want.cpu()[i].item()}")
 
 
 def check_gemm(build, dev, run=None):
     """build(dev) -> (calls [(a, w, kwargs)], outputs [tensors]): the same case built twice from its seed, once on the
     host for the reference, once on `dev` for the launch (one problem: ops.gemm, several: ops.gemm_grouped)."""
-    ops = _ops()
+    ops = mtt_ops()
     calls_ref, outs_ref = build("cpu")
     for a, w, kw in calls_ref:
         ref_gemm(a, w, **kw)
@@ -205,59 +48,13 @@ def check_gemm(build, dev, run=None):
     if dev != "cpu":
         torch.cuda.synchronize()
     for i, (got, want) in enumerate(zip(outs, outs_ref)):
-        _assert_bits_equal(got, want, f"output {i}")
-
-
-# ------------------------------------------------------------------------------------------------------------------
-# case builders (each is a function of the device; the operands come from a fixed seed on the host)
-# ------------------------------------------------------------------------------------------------------------------
-def plain_case(M, N, K, *, nsplit=2, w_nsplit=None, bias=True, act=0, residual=False, inplace=False, seed=0,
-               a_lo_zero=False, out_split_nsplit=2):
-    """One GEMM into a sentinel fp32 output and a sentinel split output with pad columns [N, ld)."""
-    w_nsplit = nsplit if w_nsplit is None else w_nsplit
-
-    def build(dev):
-        g = torch.Generator().manual_seed(seed * 7919 + M * 31 + N * 7 + K)
-        r = _range(K)
-        a = _split(dev, g, M, K, r, nsplit, lo_zero=a_lo_zero)
-        w = _split(dev, g, N, K, r, w_nsplit)
-        kw = dict(act=act)
-        if bias:
-            kw["bias"] = _ints(g, (N,), 64).to(dev)
-        of = _sentinel_f32(dev, M, N)
-        if residual:
-            res = _ints(g, (M, N), 4096).to(dev)
-            if inplace:
-                of.copy_(res)
-                res = of
-            kw["residual"] = res
-        osp = _sentinel_split(dev, M, N, out_split_nsplit, ld=(N + 7) // 8 * 8)
-        kw.update(out_f32=of, out_split=osp)
-        return [(a, w, kw)], [of, osp.buf]
-    return build
-
-
-def conv_case(B, H, W, Cin, Cout, ks, dil, *, nsplit=2, residual=False, seed=0, a_lo_zero=False):
-    def build(dev):
-        g = torch.Generator().manual_seed(seed * 104729 + B * 1000003 + H * 1009 + W * 17 + Cin * 3 + Cout + ks + dil)
-        r = _range(ks * ks * Cin)
-        M = B * H * W
-        a = _split(dev, g, M, Cin, r, nsplit, lo_zero=a_lo_zero)
-        w = _conv_weight(dev, g, Cout, Cin, ks, r, nsplit)
-        of = _sentinel_f32(dev, M, Cout)
-        osp = _sentinel_split(dev, M, Cout, 2)
-        kw = dict(N=Cout, K=Cin, bias=_ints(g, (Cout,), 64).to(dev), act=2, out_f32=of, out_split=osp,
-                  conv=(B, H, W, ks, dil))
-        if residual:
-            kw["residual"] = _ints(g, (M, Cout), 4096).to(dev)
-        return [(a, w, kw)], [of, osp.buf]
-    return build
+        assert_bits_equal(got, want, f"output {i}")
 
 
 @pytest.fixture(params=[1, 2], ids=["bn128", "bn256"])
 def tile(request, cuda_dev):
     """The GEMM's 128 x 128 (1) or 128 x 256 (2) tile, forced."""
-    ops = _ops()
+    ops = mtt_ops()
     ops.set_gemm_variant(request.param)
     try:
         yield request.param
@@ -327,14 +124,14 @@ def k_slice_case(a_lo_zero=False):
 
     def build(dev):
         g = torch.Generator().manual_seed(21)
-        r = _range(K)
-        a = _split("cpu", g, M, K0 + K + 40, r, lo_zero=a_lo_zero)
-        w = _split("cpu", g, N, K0 + K + 40, r)
+        r = int_range(K)
+        a = int_split("cpu", g, M, K0 + K + 40, r, lo_zero=a_lo_zero)
+        w = int_split("cpu", g, N, K0 + K + 40, r)
         for sp in (a, w):
             sp.buf[:, :, :K0] = float("nan")
             sp.buf[:, :, K0 + K:] = float("nan")
-        a, w = _to(a, dev), _to(w, dev)
-        of = _sentinel_f32(dev, M, N)
+        a, w = to_dev(a, dev), to_dev(w, dev)
+        of = sentinel((M, N), dev=dev)
         return [(a, w, dict(M=M, N=N, K=K, a_col_offset=K0, w_col_offset=K0, out_f32=of))], [of]
     return build
 
@@ -345,14 +142,14 @@ def row_offset_case(a_lo_zero=False):
 
     def build(dev):
         g = torch.Generator().manual_seed(22)
-        r = _range(K)
-        a = _split("cpu", g, 3 * M, K, r, lo_zero=a_lo_zero)
-        w = _split("cpu", g, 3 * N, K, r)
+        r = int_range(K)
+        a = int_split("cpu", g, 3 * M, K, r, lo_zero=a_lo_zero)
+        w = int_split("cpu", g, 3 * N, K, r)
         for sp, n in ((a, M), (w, N)):
             sp.buf[:, :n] = float("nan")
             sp.buf[:, 2 * n:] = float("nan")
-        a, w = _to(a, dev), _to(w, dev)
-        of = _sentinel_f32(dev, M, N)
+        a, w = to_dev(a, dev), to_dev(w, dev)
+        of = sentinel((M, N), dev=dev)
         return [(a, w, dict(M=M, N=N, K=K, a_row_offset=M, w_row_offset=N, out_f32=of))], [of]
     return build
 
@@ -363,27 +160,10 @@ def pad_columns_case(a_lo_zero=False):
 
     def build(dev):
         g = torch.Generator().manual_seed(23)
-        a = _split(dev, g, M, K, _range(K), ld=80, pad=float("nan"), lo_zero=a_lo_zero)
-        w = _split(dev, g, N, K, _range(K), ld=80, pad=float("nan"))
-        of = _sentinel_f32(dev, M, N)
-        return [(a, w, dict(out_f32=of, bias=_ints(g, (N,), 64).to(dev)))], [of]
-    return build
-
-
-def gather_case(G, T, stride, N=72, K=136, a_lo_zero=False):
-    """token_trans-style gathered A: rows (g, i) at g * stride + i, i < T; every row that is not gathered is NaN."""
-    def build(dev):
-        g = torch.Generator().manual_seed(24 + T)
-        a = _split("cpu", g, G * stride, K, _range(K), lo_zero=a_lo_zero)
-        keep = torch.zeros(G * stride, dtype=torch.bool)
-        keep[(torch.arange(G)[:, None] * stride + torch.arange(T)[None]).reshape(-1)] = True
-        a.buf[:, ~keep] = float("nan")
-        a = _to(a, dev)
-        w = _split(dev, g, N, K, _range(K))
-        of = _sentinel_f32(dev, G * T, N)
-        osp = _sentinel_split(dev, G * T, N)
-        return [(a, w, dict(M=G * T, a_gather=(T, stride), bias=_ints(g, (N,), 64).to(dev), out_f32=of,
-                            out_split=osp))], [of, osp.buf]
+        a = int_split(dev, g, M, K, int_range(K), ld=80, pad=float("nan"), lo_zero=a_lo_zero)
+        w = int_split(dev, g, N, K, int_range(K), ld=80, pad=float("nan"))
+        of = sentinel((M, N), dev=dev)
+        return [(a, w, dict(out_f32=of, bias=ints(g, (N,), 64).to(dev)))], [of]
     return build
 
 
@@ -405,23 +185,6 @@ def test_gathered_a(cuda_dev, tile, G, T, stride):
 # ------------------------------------------------------------------------------------------------------------------
 # 3. output addressing: every output byte outside the problem keeps its sentinel
 # ------------------------------------------------------------------------------------------------------------------
-def regroup_case(regroup, M=300, N=136, K=72, res_row_mod=0, a_lo_zero=False):
-    ig, og = regroup[:2]
-
-    def build(dev):
-        g = torch.Generator().manual_seed(31 + og)
-        rows_out = (M // ig) * og
-        a = _split(dev, g, M, K, _range(K), lo_zero=a_lo_zero)
-        w = _split(dev, g, N, K, _range(K))
-        of = _sentinel_f32(dev, rows_out, N)
-        osp = _sentinel_split(dev, rows_out, N)
-        kw = dict(bias=_ints(g, (N,), 64).to(dev), out_f32=of, out_split=osp, regroup=regroup)
-        if res_row_mod:
-            kw.update(residual=_ints(g, (res_row_mod, N), 4096).to(dev), res_row_mod=res_row_mod)
-        return [(a, w, kw)], [of, osp.buf]
-    return build
-
-
 def out_offset_case(a_lo_zero=False):
     """The split output is a window of a wider buffer: out_row_offset 3, out_col_offset 24 (like a task's columns of a
     concatenated map), split pad columns [N, ld) of a second split output."""
@@ -429,10 +192,10 @@ def out_offset_case(a_lo_zero=False):
 
     def build(dev):
         g = torch.Generator().manual_seed(33)
-        a = _split(dev, g, M, K, _range(K), lo_zero=a_lo_zero)
-        w = _split(dev, g, N, K, _range(K))
-        big = _sentinel_split(dev, M + 7, N + 40)
-        of = _sentinel_f32(dev, M, N + 9)
+        a = int_split(dev, g, M, K, int_range(K), lo_zero=a_lo_zero)
+        w = int_split(dev, g, N, K, int_range(K))
+        big = sentinel_split(M + 7, N + 40, dev)
+        of = sentinel((M, N + 9), dev=dev)
         return [(a, w, dict(N=N, out_split=big, out_row_offset=3, out_col_offset=24, out_f32=of[:, :N]))], [big.buf, of]
     return build
 
@@ -474,11 +237,11 @@ def grouped_case(count, M=130, N=136, K=72, a_lo_zero=False):
         g = torch.Generator().manual_seed(40 + count)
         calls, outs = [], []
         for _ in range(count):
-            a = _split(dev, g, M, K, _range(K), lo_zero=a_lo_zero)
-            w = _split(dev, g, N, K, _range(K))
-            of = _sentinel_f32(dev, M, N)
-            osp = _sentinel_split(dev, M, N)
-            calls.append((a, w, dict(bias=_ints(g, (N,), 64).to(dev), act=2, residual=_ints(g, (M, N), 4096).to(dev),
+            a = int_split(dev, g, M, K, int_range(K), lo_zero=a_lo_zero)
+            w = int_split(dev, g, N, K, int_range(K))
+            of = sentinel((M, N), dev=dev)
+            osp = sentinel_split(M, N, dev)
+            calls.append((a, w, dict(bias=ints(g, (N,), 64).to(dev), act=2, residual=ints(g, (M, N), 4096).to(dev),
                                      out_f32=of, out_split=osp)))
             outs += [of, osp.buf]
         return calls, outs
@@ -492,14 +255,14 @@ def upembed_case(T=3, B=2, h=6, w=10, Cin=40, Ci=72, a_lo_zero=False):
 
     def build(dev):
         g = torch.Generator().manual_seed(50)
-        r = _range(9 * Cin)
-        skip = _ints(g, (B * hw, Ci), 4096).to(dev)
-        xj = _sentinel_f32(dev, T * B * hw + 5, Ci)
+        r = int_range(9 * Cin)
+        skip = ints(g, (B * hw, Ci), 4096).to(dev)
+        xj = sentinel((T * B * hw + 5, Ci), dev=dev)
         calls = []
         for k in range(T):
-            a = _split(dev, g, B * hw, Cin, r, lo_zero=a_lo_zero)
-            wt = _conv_weight(dev, g, Ci, Cin, 3, r)
-            calls.append((a, wt, dict(N=Ci, K=Cin, bias=_ints(g, (Ci,), 64).to(dev), act=2, residual=skip,
+            a = int_split(dev, g, B * hw, Cin, r, lo_zero=a_lo_zero)
+            wt = conv_weight(dev, g, Ci, Cin, 3, r)
+            calls.append((a, wt, dict(N=Ci, K=Cin, bias=ints(g, (Ci,), 64).to(dev), act=2, residual=skip,
                                       res_row_mod=B * hw, out_f32=xj[k * hw:], regroup=(hw, T * hw, 0),
                                       conv=(B, h, w, 3, 2))))
         return calls, [xj]
@@ -520,7 +283,7 @@ def test_grouped_upembed(cuda_dev, tile):
 @pytest.mark.gpu
 def test_grouped_count_limit(cuda_dev):
     """33 problems are refused on the host with the library's error; nothing is launched."""
-    ops = _ops()
+    ops = mtt_ops()
     calls, _ = grouped_case(2, M=8, N=8, K=8)(cuda_dev)
     with pytest.raises(RuntimeError, match="33 problems"):
         ops.gemm_grouped([calls[0]] * 33)
@@ -566,7 +329,7 @@ def _streamk_geometry(M, N, K, conv=None):
 def _run_streamk(dev, geometry, mid_tap):
     """Runs the case on the stream-K schedule; before the launch, the library's own schedule for the case's geometry
     must split some tile along K (and, for mid_tap, start a piece inside a filter tap)."""
-    ops = _ops()
+    ops = mtt_ops()
     tiles, k_iters, num_kb = geometry
     ws = ops.streamk_workspace(dev)
 
@@ -638,19 +401,19 @@ ATTN = [(1, 1, 1, 1), (2, 1, 2, 2), (1, 2, 63, 5), (2, 1, 64, 1), (1, 1, 65, 5),
 def test_attention_prompt_logits(cuda_dev, nsplit, B, H, N, T):
     """The exported raw logits of the first T query rows are exactly the integer q.k^T (three-term or one-term); the
     rest of the export buffer keeps its sentinel. B = 5, H = 16 at N = 1029: more items than one wave of CTAs."""
-    ops = _ops()
+    ops = mtt_ops()
     g = torch.Generator().manual_seed(70 + N)
-    qkv = _split(cuda_dev, g, B * N, 3 * H * 64, 16, nsplit)
+    qkv = int_split(cuda_dev, g, B * N, 3 * H * 64, 16, nsplit)
     out = ops.Split(B * N, H * 64, cuda_dev, nsplit)
-    big = torch.full((B * H * T * N + 64,), float("nan"), device=cuda_dev)
+    big = sentinel((B * H * T * N + 64,), dev=cuda_dev)
     logits = big[:B * H * T * N].view(B, H, T, N) if T else None
     ops.attention(qkv, out, B=B, N=N, H=H, scale=0.125, prompt_logits=logits, T=T)
     torch.cuda.synchronize()
     s, _, _ = _logits(qkv, B, N, H, nsplit)
-    want = torch.full_like(big.cpu(), float("nan"))
+    want = sentinel(big.shape, dev="cpu")
     if T:
         want[:B * H * T * N] = s[:, :, :T, :].reshape(-1).float()
-    _assert_bits_equal(big, want, "prompt logits")
+    assert_bits_equal(big, want, "prompt logits")
     assert not torch.isnan(out.hi.float()).any()
 
 
@@ -696,15 +459,15 @@ def _retrieval_qkv(dev, B, N, H, nsplit, winners, negative):
                 k[0, b, :, h], k[1, b, :, h] = kh, k_eff - kh
             else:
                 q[0, b, :, h], k[0, b, :, h] = q_eff, k_eff
-                q[1, b, :, h] = _ints(g, (N, 64), 200)     # ignored in speed mode
-                k[1, b, :, h] = _ints(g, (N, 64), 200)
-            v[0, b, :, h] = _ints(g, (N, 64), 256)     # wide enough that means of 2 or 4 rows need a lo part
-            v[1, b, :, h] = _ints(g, (N, 64), 256)
-    ops = _ops()
+                q[1, b, :, h] = ints(g, (N, 64), 200)     # ignored in speed mode
+                k[1, b, :, h] = ints(g, (N, 64), 200)
+            v[0, b, :, h] = ints(g, (N, 64), 256)     # wide enough that means of 2 or 4 rows need a lo part
+            v[1, b, :, h] = ints(g, (N, 64), 256)
+    ops = mtt_ops()
     sp = ops.Split(B * N, 3 * H * 64, "cpu", 2)
     sp.buf.copy_(buf.bfloat16())
     assert torch.equal(sp.buf.float(), buf)
-    return _to(sp, dev)
+    return to_dev(sp, dev)
 
 
 RETRIEVAL = {
@@ -734,13 +497,13 @@ def test_attention_retrieval(cuda_dev, nsplit, case):
 def _check_retrieval(dev, case, nsplit, out_nsplit):
     """nsplit 1 with out_nsplit 1: qkv carries a junk lo plane the kernel must ignore; with out_nsplit 2: qkv has one
     plane and the output's lo plane must be written."""
-    ops = _ops()
+    ops = mtt_ops()
     assert np.float32(LN2) * np.float32(1.4426950408889634) == np.float32(1.0)
     B, N, H, winners, negative = RETRIEVAL[case]
     qkv = _retrieval_qkv(dev, B, N, H, nsplit, winners, negative)
     if nsplit == 1 and out_nsplit == 2:
         qkv.buf, qkv.nsplit = qkv.buf[:1].clone(), 1
-    out = _sentinel_split(dev, B * N, H * 64, out_nsplit)
+    out = sentinel_split(B * N, H * 64, dev, out_nsplit)
     ops.attention(qkv, out, B=B, N=N, H=H, scale=LN2)
     torch.cuda.synchronize()
 
@@ -757,11 +520,11 @@ def _check_retrieval(dev, case, nsplit, out_nsplit):
     o = (win.double() @ vv) / cnt[..., None].double()                   # [B, H, N, 64]
     o = o.permute(0, 2, 1, 3).reshape(B * N, H * 64).float()
     h_ = o.bfloat16()
-    _assert_bits_equal(out.hi, h_, "attention output hi")
+    assert_bits_equal(out.hi, h_, "attention output hi")
     if out_nsplit == 2:
         lo_want = (o - h_.float()).bfloat16()
         assert bool((lo_want != 0).any()), "the case must need a lo part"
-        _assert_bits_equal(out.lo, lo_want, "attention output lo")
+        assert_bits_equal(out.lo, lo_want, "attention output lo")
 
 
 # ------------------------------------------------------------------------------------------------------------------

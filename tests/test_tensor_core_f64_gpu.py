@@ -34,7 +34,7 @@ on the kernel's arithmetic (gemm_tc.cu mma_piece, gemm_common.cuh epilogue_op):
   * fold: stage sums P_s are added to the tile's fp32 sum with round-to-nearest; stream-K pieces start from zero and
     their partials are added in CTA order; gemm_splitk's reduction (mtt_sum_partials) starts from the bias and adds
     its K-slices in a fixed order, so there the bias is one more term of the sum. Depth at most 2 (stages) + 1
-    (+ slices + 1), so sum_tol(depth, sum_s |P_s| (+ |bias|)) (Higham & Mary, as the sibling f64 files use it).
+    (+ slices + 1), so sum_tol(depth, sum_s |P_s| (+ |bias|)) (tests/f64_checks.py).
   * the float64 reference's own rounding: cuBLAS sums each stage's at most 64 products and the stages are added one
     by one, so it is off by at most (64 + stages) 2^-53 of the absolute sum, which the chain weights (all >= 1)
     bound from above: F64_REF (64 + stages) chain. The float64 softmax and P.V of the attention reference carry
@@ -45,7 +45,7 @@ on the kernel's arithmetic (gemm_tc.cu mma_piece, gemm_common.cuh epilogue_op):
   * outputs: fp32 within the bound; when a split output is written beside it, hi = RN_bf16(out_f32) and
     lo = RN_bf16(out_f32 - hi) bit for bit; a split output alone within the bound + SPLIT |ref| + SPLIT_ABS.
 
-Attention (attention5_tc.cu) follows test_swin_kernels_gpu.py's model: a logit off by d moves a softmax weight by at
+Attention (attention5_tc.cu) follows the window-attention model of tests/kernel_cases.py: a logit off by d moves a softmax weight by at
 most a factor exp(2 d). d is the QK^T chain bound above (one 64-deep stage) times the scale, plus 3 u of the largest
 scaled logit (scale * log2 e rounded, the FMA against the running maximum, the maximum itself). Each weight further
 carries ex2.approx's relative error (2^-21) once for itself and once per running-maximum rescale (at most one per key
@@ -79,13 +79,11 @@ flags more (with q x 1 at N = 8195 the speed-mode weight errors average out over
 with q x 12 a few keys carry each row and they do not). The worst err / bound ratio per config and kind, and the
 fraction each teeth check flagged, are printed.
 
-The CPU self-checks (no GPU) run the reference builder on integer planes against test_tc_exact_gpu.ref_gemm bit for
+The CPU self-checks (no GPU) run the reference builder on integer planes against tests/kernel_cases.py ref_gemm bit for
 bit, a CPU model of the kernel's arithmetic (fp32 chains truncated after every k16 step, round-to-nearest fold)
 against the bound, and the key builder.
 """
 import collections
-import contextlib
-import inspect
 import math
 import time
 
@@ -93,8 +91,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from test_tc_exact_gpu import _out_rows, _sentinel_split
-from test_train_kernels_f64_gpu import SPLIT, SPLIT_ABS, U, check, sum_tol
+import kernel_cases as X
+from f64_checks import (SENTINEL, SPLIT, SPLIT_ABS, U, bits, check, mtt_ops, planes, sentinel, sentinel_split,
+                        split_bound, sum_tol)
+from plan_calls import frozen, recording
 
 pytestmark = [pytest.mark.timeout(1500)]   # the GPU tests are marked one by one: the CPU self-checks are not
 
@@ -104,19 +104,11 @@ EX2 = 2.0 ** -21          # relative error of ex2.approx.ftz.f32
 F64_REF = 2.0 ** -53      # float64 unit roundoff: the reference's own rounding (see the docstring)
 TEETH_FRAC = 0.10
 TAIL_STAGES = 32          # keys with at most this many K-stages must show the ragged-tail defect (see the docstring)
-F32_SENT = 0x7FC0BEEF     # one fixed NaN payload, so that an untouched element keeps its exact bits
-BF16_SENT = 0x7FA5        # the pattern test_tc_exact_gpu._sentinel_split writes
 FORWARD = ["tp_cfg4", "tp_cfg2", "tp_cfg5", "ip_cfg3", "tps_swinB", "tps_swinB3d"]
 EXTRA_BATCH = {"tps_swinB3d": 1}   # forwards the bench does not run: their batch
 TRAIN = ["tp_cfg4", "tp_cfg2"]
 RECORDED = ["gemm", "gemm_grouped", "gemm_splitk", "attention", "ln_qkv", "proj_residual", "ln_mlp_residual",
             "gated_conv1x1", "conv3x3_bn_act"]
-
-
-def _ops():
-    import mtt_b200  # noqa: F401
-    from mtt_b200 import ops
-    return ops
 
 
 def cdiv(a, b):
@@ -142,10 +134,6 @@ def _tg(t):
     return None if t is None else (int(t.shape[-2]), int(t.shape[-1]), int(t.stride(-2)))
 
 
-def _frozen(d):
-    return tuple(sorted(d.items()))
-
-
 def gemm_fields(a, w, kw, sk_ws=None):
     """The geometry of one ops.gemm problem: everything that selects a code path or an address."""
     g = dict(kw)
@@ -161,7 +149,7 @@ def gemm_fields(a, w, kw, sk_ws=None):
         rk = "separate"
     osp = g.get("out_split")
     regroup, gather, conv = g.get("regroup"), g.get("a_gather"), g.get("conv")
-    return _frozen(dict(
+    return frozen(dict(
         M=int(a.rows if g.get("M") is None else g["M"]), N=int(w.rows if g.get("N") is None else g["N"]),
         K=int(a.cols if g.get("K") is None else g["K"]), nsplit=ns, conv=None if conv is None else tuple(conv),
         act=int(g.get("act", 0)), bias=g.get("bias") is not None, res=rk, res_row_mod=int(g.get("res_row_mod", 0)),
@@ -182,33 +170,33 @@ def call_key(fn, args):
     if fn == "gemm_grouped":
         return ("gemm", tuple(gemm_fields(a, w, kw) for a, w, kw in A["calls"]))
     if fn == "gemm_splitk":
-        return ("splitk", _frozen(dict(a=_sg(A["a"]), w=_sg(A["w"]), partial=tuple(A["partial"].shape),
+        return ("splitk", frozen(dict(a=_sg(A["a"]), w=_sg(A["w"]), partial=tuple(A["partial"].shape),
                                        out_f32=_tg(A["out_f32"]), K=int(A["K"]), chunks=int(A["chunks"]),
                                        bias=A["bias"] is not None, nsplit=min(A["a"].nsplit, A["w"].nsplit))))
     if fn == "attention":
         pl = A["prompt_logits"]
-        return ("attention", _frozen(dict(B=A["B"], N=A["N"], H=A["H"], T=int(A["T"]), scale=float(A["scale"]),
+        return ("attention", frozen(dict(B=A["B"], N=A["N"], H=A["H"], T=int(A["T"]), scale=float(A["scale"]),
                                           qkv=_sg(A["qkv"]), out=_sg(A["out"]), logits=pl is not None,
                                           nsplit=min(A["qkv"].nsplit, A["out"].nsplit))))
     if fn == "ln_qkv":
-        return ("ln_qkv", _frozen(dict(x=_tg(A["x"]), w=_sg(A["wqkv"]), qkv=_sg(A["qkv"]),
+        return ("ln_qkv", frozen(dict(x=_tg(A["x"]), w=_sg(A["wqkv"]), qkv=_sg(A["qkv"]),
                                        nsplit=min(A["wqkv"].nsplit, A["qkv"].nsplit))))
     if fn == "proj_residual":
-        return ("proj_residual", _frozen(dict(x=_tg(A["x"]), a=_sg(A["ao"]), w=_sg(A["wproj"]),
+        return ("proj_residual", frozen(dict(x=_tg(A["x"]), a=_sg(A["ao"]), w=_sg(A["wproj"]),
                                               nsplit=min(A["ao"].nsplit, A["wproj"].nsplit))))
     if fn == "ln_mlp_residual":
-        return ("ln_mlp_residual", _frozen(dict(x=_tg(A["x"]), w1=_sg(A["w1"]), w2=_sg(A["w2"]),
+        return ("ln_mlp_residual", frozen(dict(x=_tg(A["x"]), w1=_sg(A["w1"]), w2=_sg(A["w2"]),
                                                 nsplit=min(A["w1"].nsplit, A["w2"].nsplit))))
     if fn == "gated_conv1x1":
         t0 = A["tasks"][0]
-        return ("gated_conv1x1", _frozen(dict(
+        return ("gated_conv1x1", frozen(dict(
             x=tuple(A["x"].shape) + (int(A["x"].stride(-2)),), x_group_rows=int(A["x_group_rows"]),
             x_row_offset=int(A["x_row_offset"]), logits=tuple(A["prompt_logits"].shape),
             chan_lg=tuple(A["chan_lg"].shape), ntasks=len(A["tasks"]), e=int(A["e"]), chan_col=int(A["chan_col"]),
             w_spa=_sg(t0[0]), w_chan=_sg(t0[2]), cat=_sg(t0[4]), nsplit=min(t0[0].nsplit, t0[4].nsplit),
             shape=tuple(int(A[k]) for k in ("B", "T", "N", "H", "Cdim", "gh", "gw", "nh", "nw")))))
     if fn == "conv3x3_bn_act":
-        return ("conv3x3_bn_act", _frozen(dict(
+        return ("conv3x3_bn_act", frozen(dict(
             a=_sg(A["a"]), w3=_sg(A["w3"]), Cin=int(A["Cin"]), Cout=int(A["Cout"]), act=int(A["act"]),
             conv=(int(A["B"]), int(A["H"]), int(A["W"]), int(A["dil"])), mid=_sg(A["mid"]), w_head=_sg(A["w_head"]),
             n_out=int(A["n_out"]), out_f32=_tg(A["out_f32"]), nsplit=min(A["a"].nsplit, A["w3"].nsplit))))
@@ -267,33 +255,6 @@ def launches_of(key):
     raise KeyError(kind)
 
 
-@contextlib.contextmanager
-def recording(ops, seen):
-    """Pass-through recorders around RECORDED; calls made from inside a recorded call (gemm_splitk's grouped launch)
-    belong to the outer call."""
-    depth = [0]
-    mp = pytest.MonkeyPatch()
-    for fn in RECORDED:
-        orig = getattr(ops, fn)
-        sig = inspect.signature(orig)
-
-        def rec(*a, _fn=fn, _orig=orig, _sig=sig, **k):
-            if depth[0] == 0:
-                ba = _sig.bind(*a, **k)
-                ba.apply_defaults()
-                seen.append(call_key(_fn, ba.arguments))
-            depth[0] += 1
-            try:
-                return _orig(*a, **k)
-            finally:
-                depth[0] -= 1
-        mp.setattr(ops, fn, rec)
-    try:
-        yield
-    finally:
-        mp.undo()
-
-
 # ---- float64 references ------------------------------------------------------------------------------------------------
 def _stage_cols(K, P):
     """Per product kind (P of them), the chain weight n_s - j(k) of every column k of one K-long block (a GEMM, or one
@@ -305,10 +266,6 @@ def _stage_cols(K, P):
     nsteps = torch.where(s == nkb - 1, torch.full_like(s, last), torch.full_like(s, 4)) * P
     ks = (k % 64) // 16
     return [(nsteps - (ks * P + kind)).double() for kind in range(P)]
-
-
-def _planes(sp, ns):
-    return [sp.buf[0]] + ([sp.buf[1]] if ns == 2 else [])
 
 
 def gemm_ref(spec, tail=False):
@@ -338,7 +295,7 @@ def gemm_ref(spec, tail=False):
             x = F.pad(p[rows, aco:aco + K].double().reshape(B, H, W, K), (0, 0, pd, pd, pd, pd))
             ky, kx = t
             return x[:, ky * dil:ky * dil + H, kx * dil:kx * dil + W, :].reshape(M, K)
-    Ap, Wp = _planes(a, ns), _planes(w, ns)
+    Ap, Wp = planes(a, ns), planes(w, ns)
     y = torch.zeros(M, N, dtype=torch.float64, device=dev)
     chain, absP = torch.zeros_like(y), torch.zeros_like(y)
     tl = torch.zeros_like(y) if tail else None
@@ -381,10 +338,6 @@ def epilogue(v, E, bias, act, res):
     return v, E
 
 
-def _bits(t):
-    return t.view(torch.int32) if t.dtype == torch.float32 else t.view(torch.int16)
-
-
 def stage_check(spec, teeth=None):
     """Check one GEMM stage's outputs against its reference and bound. spec also holds bias (fp32 or None), act,
     res (float64 [M, N] as consumed, or None) and outs: [("f32", tensor, rows, col0) | ("split", Split, rows, col0)].
@@ -413,15 +366,14 @@ def stage_check(spec, teeth=None):
             got = buf.buf[0][rows, c0:c0 + N].double()
             if buf.nsplit == 2:
                 got = got + buf.buf[1][rows, c0:c0 + N].double()
-            rel = SPLIT if buf.nsplit == 2 else 2.0 ** -8
-            bnd = bound + rel * (ref.abs() + bound) + SPLIT_ABS
+            bnd = bound + split_bound(buf.nsplit, ref.abs() + bound)
             if f32 and teeth is None:       # both outputs: the split is the RN split of the fp32 value, bit for bit
                 o32 = f32[0][1][f32[0][2].to(ref.device), f32[0][3]:f32[0][3] + N]
                 hi = o32.bfloat16()
-                assert torch.equal(_bits(buf.buf[0][rows, c0:c0 + N]), _bits(hi)), "split hi != RN_bf16(out_f32)"
+                assert torch.equal(bits(buf.buf[0][rows, c0:c0 + N]), bits(hi)), "split hi != RN_bf16(out_f32)"
                 if buf.nsplit == 2:
                     lo = (o32 - hi.float()).bfloat16()
-                    assert torch.equal(_bits(buf.buf[1][rows, c0:c0 + N]), _bits(lo)), "split lo != RN_bf16(out - hi)"
+                    assert torch.equal(bits(buf.buf[1][rows, c0:c0 + N]), bits(lo)), "split lo != RN_bf16(out - hi)"
         if teeth is None:
             worst = max(worst, check(got, ref, bnd, f"{spec['what']} {kind}"))
             continue
@@ -445,9 +397,9 @@ def attn_ref(qkv, B, N, H, ns, scale, b, heads):
     C = H * 64
     rows = slice(b * N, (b + 1) * N)
     part = lambda p, off: p[rows, off:off + C].double().view(N, H, 64)[:, heads].permute(1, 0, 2)
-    Pq = [part(p, 0) for p in _planes(qkv, ns)]
-    Pk = [part(p, C) for p in _planes(qkv, ns)]
-    Pv = [part(p, 2 * C) for p in _planes(qkv, 2)]
+    Pq = [part(p, 0) for p in planes(qkv, ns)]
+    Pk = [part(p, C) for p in planes(qkv, ns)]
+    Pv = [part(p, 2 * C) for p in planes(qkv, 2)]
     P = 3 if ns == 2 else 1
     pairs = [(0, 0), (0, 1), (1, 0)][:P]
     wts = [t.to(qkv.buf.device) for t in _stage_cols(64, P)]
@@ -492,26 +444,19 @@ class Draw:
         x = self.randn(rows, ld) * self.rowscale(rows)
         for c0, c1 in zero_cols or ():
             x[:, c0:c1] = 0
-        sp = _ops().split_f32(x)
+        sp = mtt_ops().split_f32(x)
         sp.cols = cols
         return sp
 
 
 def hi_only(sp):
-    return _ops().Split.from_planes(sp.buf[:1], sp.cols)
+    return mtt_ops().Split.from_planes(sp.buf[:1], sp.cols)
 
 
-def sentinel_f32(rows, ld, dev):
-    """Like test_tc_exact_gpu._sentinel_f32, but with one fixed NaN payload: Outputs.untouched compares bits."""
-    t = torch.empty(rows, ld, device=dev)
-    t.view(torch.int32).fill_(F32_SENT)
-    return t
-
-
-def sentinel_split(geom, dev):
+def sentinel_of(geom, dev):
     """A sentinel-filled Split of a recorded (rows, cols, ld, planes) geometry."""
-    rows, cols, ld, planes = geom
-    return _sentinel_split(dev, rows, cols, planes, ld=ld)
+    rows, cols, ld, ns = geom
+    return sentinel_split(rows, cols, dev, ns, ld=ld)
 
 
 def conv_weight_zeros(K, taps, wco):
@@ -521,7 +466,7 @@ def conv_weight_zeros(K, taps, wco):
 
 def tail_zeroed(w, K, taps, wco):
     """A copy of W whose lo plane is zero in the last K-stage of every tap."""
-    ops = _ops()
+    ops = mtt_ops()
     sp = ops.Split.from_planes(w.buf.clone(), w.cols)
     cp = cdiv(K, 64) * 64 if taps > 1 else K
     k0 = 64 * (cdiv(K, 64) - 1)
@@ -548,7 +493,7 @@ class Outputs:
 
     def untouched(self, what):
         for buf, init, m in self.items:
-            same = _bits(buf) == _bits(init)
+            same = bits(buf) == bits(init)
             bad = ~m & ~same
             assert not bad.any(), f"{what}: {int(bad.sum())} elements outside the output written"
 
@@ -584,11 +529,11 @@ class Case:
         bias = d.randn(N) if f["bias"] else None
         kw["bias"] = bias
         r = torch.arange(M, device=dev)
-        ro = _out_rows(r, f["regroup"])
+        ro = X.out_rows(r, f["regroup"])
         outs, res = [], None
         if f["out_f32"] is not None:
             rows, cols, ld = f["out_f32"]
-            buf = sentinel_f32(rows, ld, dev)
+            buf = sentinel((rows, ld), dev=dev)
             if f["res"] == "inplace":
                 buf.copy_(d.randn(rows, ld))
             m = self.out.add(buf)
@@ -605,7 +550,7 @@ class Case:
             kw["residual"] = kw["out_f32"]
             res = self.out.items[-1][1][ro, :N].double()
         if f["out_split"] is not None:
-            osp = sentinel_split(f["out_split"], dev)
+            osp = sentinel_of(f["out_split"], dev)
             m = self.out.add(osp.buf)
             m[:, (ro + oro)[:, None], oco + torch.arange(N, device=dev)[None]] = True
             kw["out_split"] = osp
@@ -620,11 +565,11 @@ class Case:
 
     def _build_gemm(self, body):
         self.probs = [self._problem(p) for p in body]
-        self.sk = _ops().streamk_workspace(self.dev) if self.probs[0][5] else None
+        self.sk = mtt_ops().streamk_workspace(self.dev) if self.probs[0][5] else None
         self.K, self.taps = self.probs[0][3]["K"], self.probs[0][4]
 
     def _run_gemm(self, ns, tail):
-        ops = _ops()
+        ops = mtt_ops()
         calls = []
         for a, w, kw, spec, taps, _ in self.probs:
             if tail:
@@ -648,7 +593,7 @@ class Case:
         M, N, K = f["a"][0], f["w"][0], f["K"]
         self.partial = torch.empty(f["partial"], device=dev)
         rows, cols, ld = f["out_f32"]
-        buf = sentinel_f32(rows, ld, dev)
+        buf = sentinel((rows, ld), dev=dev)
         m = self.out.add(buf)
         m[:M, :N] = True
         self.o32 = buf[:, :cols]
@@ -662,7 +607,7 @@ class Case:
         a, w = self.a, tail_zeroed(self.w, self.K, 1, 0) if tail else self.w
         if ns == 1:
             a, w = hi_only(a), hi_only(w)
-        _ops().gemm_splitk(a, w, self.partial, self.o32, K=self.K, bias=self.bias, chunks=self.chunks)
+        mtt_ops().gemm_splitk(a, w, self.partial, self.o32, K=self.K, bias=self.bias, chunks=self.chunks)
 
     def _specs_splitk(self, ns):
         return [dict(self.spec, a=self.a, w=self.w, ns=ns)]
@@ -678,18 +623,18 @@ class Case:
 
     def _build_ln_qkv(self, body):
         f = dict(body)
-        ops, d, dev = _ops(), self.draw, self.dev
+        ops, d, dev = mtt_ops(), self.draw, self.dev
         rows, C = f["x"][:2]
         self.xbuf, self.x = self._x(f["x"])
         self.g, self.b = self._ln(C)
         self.w, self.bias = d.split(f["w"]), d.randn(3 * C)
-        self.qkv = sentinel_split(f["qkv"], dev)
+        self.qkv = sentinel_of(f["qkv"], dev)
         m = self.out.add(self.qkv.buf)
         m[:, :rows, :3 * C] = True
         self.rows, self.C, self.K, self.taps = rows, C, C, 1
 
     def _run_ln_qkv(self, ns, tail):
-        ops = _ops()
+        ops = mtt_ops()
         w = tail_zeroed(self.w, self.C, 1, 0) if tail else self.w
         w = hi_only(w) if ns == 1 else w
         self.ws = ops.workspace(ops.workspace_bytes(ops.OP_LN_QKV, rows=self.rows, Cdim=self.C, nsplit=ns), self.dev)
@@ -697,7 +642,7 @@ class Case:
 
     def _specs_ln_qkv(self, ns):
         r = torch.arange(self.rows, device=self.dev)
-        xn = _ops().ws_split_view(self.ws, 0, self.rows, self.C, ns)
+        xn = mtt_ops().ws_split_view(self.ws, 0, self.rows, self.C, ns)
         return [dict(a=xn, w=self.w, ns=ns, M=self.rows, N=3 * self.C, K=self.C, conv=None, arow=r, bias=self.bias,
                      act=0, res=None, outs=[("split", self.qkv, r, 0)], what="ln_qkv")]
 
@@ -716,7 +661,7 @@ class Case:
         a, w = self.a, tail_zeroed(self.w, self.C, 1, 0) if tail else self.w
         if ns == 1:
             a, w = hi_only(a), hi_only(w)
-        _ops().proj_residual(a, w, self.bias, self.x)
+        mtt_ops().proj_residual(a, w, self.bias, self.x)
 
     def _specs_proj_residual(self, ns):
         r = torch.arange(self.rows, device=self.dev)
@@ -737,7 +682,7 @@ class Case:
         self.rows, self.C, self.hid, self.K, self.taps = rows, C, hid, hid, 1
 
     def _run_ln_mlp_residual(self, ns, tail):
-        ops = _ops()
+        ops = mtt_ops()
         w1, w2 = self.w1, tail_zeroed(self.w2, self.hid, 1, 0) if tail else self.w2
         if ns == 1:
             w1, w2 = hi_only(w1), hi_only(w2)
@@ -746,7 +691,7 @@ class Case:
         ops.ln_mlp_residual(self.x, self.g, self.b, 1e-6, w1, self.b1, w2, self.b2, self.ws)
 
     def _specs_ln_mlp_residual(self, ns):
-        ops = _ops()
+        ops = mtt_ops()
         r = torch.arange(self.rows, device=self.dev)
         xn = ops.ws_split_view(self.ws, 0, self.rows, self.C, ns)
         h = ops.ws_split_view(self.ws, align256(2 * ns * self.rows * pad8(self.C)), self.rows, self.hid, ns)
@@ -766,7 +711,7 @@ class Case:
         self.chan = d.randn(*f["chan_lg"])
         self.tasks = []
         for _ in range(f["ntasks"]):
-            cat = sentinel_split(f["cat"], dev)
+            cat = sentinel_of(f["cat"], dev)
             m = self.out.add(cat.buf)
             m[:, :B * gh * gw, :f["e"]] = True
             m[:, :B * gh * gw, f["chan_col"]:f["chan_col"] + f["e"]] = True
@@ -774,7 +719,7 @@ class Case:
         self.f, self.rows, self.C, self.K, self.taps = f, B * gh * gw, C, C, 1
 
     def _run_gated_conv1x1(self, ns, tail):
-        ops = _ops()
+        ops = mtt_ops()
         f = self.f
         B, T, N, H, C, gh, gw, nh, nw = f["shape"]
         tasks = []
@@ -790,7 +735,7 @@ class Case:
                           f["chan_col"], self.ws, B=B, T=T, N=N, H=H, Cdim=C, gh=gh, gw=gw, nh=nh, nw=nw)
 
     def _specs_gated_conv1x1(self, ns):
-        ops = _ops()
+        ops = mtt_ops()
         r = torch.arange(self.rows, device=self.dev)
         pb = align256(2 * ns * self.rows * pad8(self.C))
         out = []
@@ -811,14 +756,14 @@ class Case:
         self.w3, self.b3 = d.split(f["w3"], conv_weight_zeros(Cin, 9, 0)), d.randn(Cout)
         self.mid = None
         if f["mid"] is not None:
-            self.mid = sentinel_split(f["mid"], dev)
+            self.mid = sentinel_of(f["mid"], dev)
             m = self.out.add(self.mid.buf)
             m[:, :M, :Cout] = True
         self.wh = self.bh = self.o32 = None
         if f["w_head"] is not None:
             self.wh, self.bh = d.split(f["w_head"]), d.randn(f["n_out"])
             rows, cols, ld = f["out_f32"]
-            self.obuf = sentinel_f32(rows, ld, dev)
+            self.obuf = sentinel((rows, ld), dev=dev)
             m = self.out.add(self.obuf)
             m[:M, :f["n_out"]] = True
             self.o32 = self.obuf[:, :cols]
@@ -826,7 +771,7 @@ class Case:
         self.K, self.taps = (Cout, 1) if self.wh is not None else (Cin, 9)
 
     def _run_conv3x3_bn_act(self, ns, tail):
-        ops = _ops()
+        ops = mtt_ops()
         f = self.f
         B, H, W, dil = f["conv"]
         a, w3, wh = self.a, self.w3, self.wh
@@ -849,7 +794,7 @@ class Case:
         f = self.f
         B, H, W, dil = f["conv"]
         r = torch.arange(self.M, device=self.dev)
-        mid = self.mid if self.mid is not None else _ops().ws_split_view(self.ws, 0, self.M, self.Cout, ns)
+        mid = self.mid if self.mid is not None else mtt_ops().ws_split_view(self.ws, 0, self.M, self.Cout, ns)
         out = [dict(a=self.a, w=self.w3, ns=ns, M=self.M, N=self.Cout, K=self.Cin, conv=(B, H, W, 3, dil), arow=r,
                     bias=self.b3,
                     act=f["act"], res=None, outs=[("split", mid, r, 0)], what=f"conv3x3 {B}x{H}x{W} {self.Cin}->{self.Cout}")]
@@ -874,7 +819,7 @@ class Case:
 def replay_gemm_key(key, dev, seed):
     """Both modes, both draws, and the teeth on the plain draw. Returns (worst ratio, [(speed-mode fraction flagged or
     None, tail fraction flagged, tail fraction detectable, K-stages)])."""
-    ops = _ops()
+    ops = mtt_ops()
     worst, teeth = 0.0, []
     for scaled in (False, True):
         case = Case(key, Draw(dev, seed + scaled, scaled), dev)
@@ -912,7 +857,7 @@ def replay_gemm_key(key, dev, seed):
 
 
 def replay_attention_key(key, dev, seed):
-    ops = _ops()
+    ops = mtt_ops()
     f = dict(key[1])
     B, N, H, T, scale = f["B"], f["N"], f["H"], f["T"], f["scale"]
     worst, teeth = {"attention": 0.0, "prompt_logits": 0.0}, []
@@ -923,13 +868,13 @@ def replay_attention_key(key, dev, seed):
         x = d.randn(B * N, 3 * H * 64)
         x[:, :H * 64] *= qs
         qkv = ops.split_f32(x)
-        out = sentinel_split(f["out"], dev)
+        out = sentinel_of(f["out"], dev)
         logits = torch.empty(B, H, T, N, device=dev) if f["logits"] else None
         results = {}
         for ns in (2, 1):
-            out.buf.view(torch.int16).fill_(BF16_SENT)
+            bits(out.buf).fill_(SENTINEL[torch.bfloat16])
             if logits is not None:
-                logits.view(torch.int32).fill_(F32_SENT)
+                bits(logits).fill_(SENTINEL[torch.float32])
             q = qkv if ns == 2 else hi_only(qkv)
             ops.attention(q, out, B=B, N=N, H=H, scale=scale, prompt_logits=logits, T=T)
             torch.cuda.synchronize()
@@ -975,7 +920,7 @@ def _record_run(ops, fn):
     seen = []
     ops.profile_begin()
     try:
-        with recording(ops, seen):
+        with recording(ops, RECORDED, call_key, seen, outermost_only=True):
             with torch.no_grad():
                 fn()
     finally:
@@ -985,7 +930,7 @@ def _record_run(ops, fn):
 
 def _forward(name, dev, nsplit):
     import bench
-    ops = _ops()
+    ops = mtt_ops()
     cfg, model = _build(name, dev, nsplit)
     model.eval()
     x = torch.randn(EXTRA_BATCH.get(name) or bench.DEFAULT_BATCH[name], 3, *cfg["img_size"], device=dev)
@@ -998,7 +943,7 @@ def _forward(name, dev, nsplit):
 def _train(name, dev):
     import bench
     from mtt_b200.train import TrainStep
-    ops = _ops()
+    ops = mtt_ops()
     cfg, model = _build(name, dev, 2)
     ts = TrainStep(model, nsplit=2, use_graph=False)
     crit, _ = bench._train_criterion(cfg)
@@ -1015,7 +960,7 @@ def _train(name, dev):
 @pytest.fixture(scope="module")
 def recorded(cuda_dev):
     """{(config, "forward" | "train" | "forward_speed"): (recorded keys in call order, profiled launches)}."""
-    _ops()
+    mtt_ops()
     runs = {}
     for name in FORWARD:
         runs[(name, "forward")] = _forward(name, cuda_dev, 2)
@@ -1056,7 +1001,7 @@ def test_speed_mode_plan_records_the_same_keys(recorded):
 
 
 def _replay_all(recorded, name, part, dev):
-    ops = _ops()
+    ops = mtt_ops()
     ops.set_gemm_variant(0)
     ops.set_gemm_streamk(1)
     keys = distinct(recorded[(name, part)][0])
@@ -1120,8 +1065,6 @@ def _spec_of_call(a, w, kw, ns):
 def test_reference_builder_matches_exact_reference():
     """On integer planes (nothing rounds) gemm_ref + epilogue equals test_tc_exact_gpu.ref_gemm bit for bit: plain,
     regrouped with a row-mod residual, gathered A, and a dilated convolution with a residual, in both modes."""
-    import test_tc_exact_gpu as X
-
     builds = [X.plain_case(129, 257, 130, residual=True, act=2, seed=5),
               X.plain_case(127, 129, 130, nsplit=1, residual=True, inplace=True),
               X.regroup_case((100, 105, 5), res_row_mod=100), X.gather_case(10, 32, 40),
@@ -1136,7 +1079,7 @@ def test_reference_builder_matches_exact_reference():
         spec = _spec_of_call(a, w, kw, ns)
         y, E, _, _ = gemm_ref(spec)
         r = torch.arange(spec["M"])
-        ro = _out_rows(r, kw.get("regroup"))
+        ro = X.out_rows(r, kw.get("regroup"))
         rv = None
         if res0 is not None:
             rr = r % kw["res_row_mod"] if kw.get("res_row_mod", 0) > 0 else ro
@@ -1145,7 +1088,7 @@ def test_reference_builder_matches_exact_reference():
         v, _ = epilogue(y, E, None if b is None else b[:spec["N"]].double()[None], kw.get("act", 0), rv)
         if kw.get("out_f32") is not None:
             want = kw["out_f32"][ro, :spec["N"]]
-            assert torch.equal(_bits(v.float()), _bits(want)), "reference builder != ref_gemm"
+            assert torch.equal(bits(v.float()), bits(want)), "reference builder != ref_gemm"
         assert float(E.max()) > 0
 
 
@@ -1177,7 +1120,7 @@ def _model_kernel(a, w, ns):
 def test_arithmetic_model_within_bound_and_speed_mode_outside():
     """The CPU model of the kernel (truncating k16 steps, RN fold) stays within gemm_ref's bound at a ragged K with
     both draws; the speed-mode model against the parity reference and bound fails on most elements."""
-    ops = _ops()
+    ops = mtt_ops()
     g = torch.Generator().manual_seed(3)
     M, N, K = 24, 40, 200
     for scaled in (False, True):
@@ -1200,7 +1143,7 @@ def test_arithmetic_model_within_bound_and_speed_mode_outside():
 
 def test_keys_tell_apart_what_selects_a_path():
     """Calls differing only in residual kind, regroup or an offset get distinct keys; identical calls one key."""
-    ops = _ops()
+    ops = mtt_ops()
     a, w = ops.Split(300, 72, "cpu"), ops.Split(136, 72, "cpu")
     out = torch.zeros(400, 136)
     res = torch.zeros(400, 136)

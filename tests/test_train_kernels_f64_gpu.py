@@ -4,38 +4,25 @@ references written from each operation's definition: torch autograd in float64 f
 clip_grad_norm_ / torch.optim.Adam in float64, oracle/loss_ref.py in float64. Then the whole tp_cfg2_d4 reverse pass
 against autograd of the train-mode restatement.
 
-Error model. u = 2^-24 is the fp32 unit roundoff. A reduction that adds terms a_i in fp32 along a tree whose longest
-chain of additions is D (per-thread serial sum + warp shuffles + shared-memory steps + atomics, counted from the kernel's
-launch geometry) is bounded by LAM * sqrt(D) * u * sum |a_i| (the probabilistic bound of Higham & Mary 2019, with
-LAM = 4 covering it at far beyond the 1 - 1e-6 level); each elementwise fp32 operation adds u relative. A value written
-as split planes (hi + lo bf16) carries a further error of 2^-17 relative or 2^-133 absolute (bf16 subnormals),
-whichever is larger. The BatchNorm statistics accumulate in double (u64 = 2^-53 in place of u). Pure data movement is
-bit-exact. Every assert below states which of these it uses."""
+Error model: tests/f64_checks.py. The BatchNorm statistics accumulate in double (U64 in place of u). Every assert below
+states which bound it uses."""
 import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
+from f64_checks import LAM, SPLIT, SPLIT_ABS, U, U64, check, gen, ops, randn, split_planes, sum_tol  # noqa: F401
 from oracle import configs, loss_ref
+from plan_calls import TPGeom
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 
-U = 2.0 ** -24            # fp32 unit roundoff
-U64 = 2.0 ** -53          # fp64 unit roundoff (the BatchNorm statistics accumulate in double)
-SPLIT = 2.0 ** -17        # relative precision of a value stored as hi + lo bf16 planes
-SPLIT_ABS = 2.0 ** -133   # ... and its absolute floor: the lo plane's spacing once it is subnormal in bf16
-LAM = 4.0                 # probabilistic summation bound: |error| <= LAM sqrt(D) u sum|a_i|
 CONFIGS = ["tp_cfg4", "tp_cfg2"]
 
 
 def _sms():
     return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def sum_tol(D, abs_sum):
-    """Bound of an fp32 reduction of depth D whose terms have absolute sum abs_sum (tensor or float)."""
-    return LAM * math.sqrt(D) * U * abs_sum
 
 
 def colreduce_depth(rows, cols):
@@ -46,64 +33,10 @@ def colreduce_depth(rows, cols):
     return math.ceil(rows / (8 * rb)) + 8 + rb
 
 
-def check(got, ref, bound, what):
-    """|got - ref| <= bound elementwise (all float64 on the device); reports the worst ratio."""
-    got, ref = got.double(), ref.double()
-    bound = torch.as_tensor(bound, dtype=torch.float64, device=ref.device).expand_as(ref)
-    err = (got - ref).abs()
-    r = err / bound.clamp_min(1e-300)
-    i = int(r.argmax())
-    ratio = r.reshape(-1)[i].item()
-    assert torch.isfinite(got).all(), f"{what}: non-finite values"
-    idx = tuple(int(k) for k in torch.unravel_index(torch.tensor(i), ref.shape))
-    assert (err <= bound).all(), (f"{what}: error {ratio:.2f}x its bound at {idx}: got {got.reshape(-1)[i].item():.9e}, "
-                                  f"want {ref.reshape(-1)[i].item():.9e}, bound {bound.reshape(-1)[i].item():.3e} "
-                                  f"(max abs err {err.max().item():.3e})")
-    return ratio
-
-
-class Geom:
-    """The training geometry of a bench config at the bench's training batch (bench.DEFAULT_BATCH)."""
-
-    def __init__(self, name):
-        import bench
-
-        cfg = configs.taskprompter(name)
-        self.name, self.cfg = name, cfg
-        self.B = bench.DEFAULT_BATCH[name]
-        self.T = len(cfg["tasks"])
-        self.gh, self.gw = cfg["img_size"][0] // cfg["patch"], cfg["img_size"][1] // cfg["patch"]
-        self.P = self.gh * self.gw
-        self.N = self.T + self.P
-        self.H, self.C = cfg["heads"], cfg["C"]
-        self.dh = self.C // self.H
-        self.nh = self.nw = int(round(math.sqrt(cfg["chan_nheads"])))
-        self.e, self.f = cfg["e"], cfg["f"]
-        self.h4, self.w4 = 4 * self.gh, 4 * self.gw
-        self.M4 = self.B * self.h4 * self.w4       # rows of the heads' mt_proj.1 BatchNorm (ConvHead at 4x the token grid)
-        self.Mp = self.B * self.P                  # rows of the decoder's fea_fuse.*.2 BatchNorm (token grid)
-        self.use_ctr = cfg["use_ctr"]
-
-
 @pytest.fixture(scope="module", params=CONFIGS)
 def geom(request, cuda_dev):
     import mtt_b200  # noqa: F401
-    return Geom(request.param)
-
-
-@pytest.fixture(scope="module")
-def ops(cuda_dev):
-    import mtt_b200  # noqa: F401
-    from mtt_b200 import ops as o
-    return o
-
-
-def gen(seed):
-    return torch.Generator(device="cuda").manual_seed(seed)
-
-
-def randn(g, *shape):
-    return torch.randn(*shape, generator=g, device="cuda", dtype=torch.float32)
+    return TPGeom(request.param)
 
 
 def split_of(ops, x):
@@ -504,12 +437,6 @@ def test_colsum_step_mappings_f64(ops, geom):
         check(out, out0.double() + rows_ref.sum(0), sum_tol(D, rows_ref.abs().sum(0) + out0.double().abs()), f"colsum {name}")
 
 
-def _split_planes_of(v):
-    """The hi / lo bf16 planes of fp32 v as the kernels write them (round to nearest even, lo = v - hi)."""
-    hi = v.bfloat16()
-    return hi, (v - hi.float()).bfloat16()
-
-
 def test_im2col_and_transpose_bit_exact(ops, geom):
     """im2col3x3_t (conv weight-gradient operand of the decoder's 3x3 convs and the heads' mt_proj.0), im2col_patch_t
     (patch embedding) and transpose_planes at the step's shapes: bit for bit against F.unfold + the split."""
@@ -519,13 +446,13 @@ def test_im2col_and_transpose_bit_exact(ops, geom):
         x = randn(g, B * H * W, f)
         got = ops.im2col3x3_t(x, B=B, H=H, W=W, Cdim=f)
         cols = F.unfold(x.view(B, H, W, f).permute(0, 3, 1, 2), 3, padding=1).permute(1, 0, 2).reshape(f * 9, B * H * W)
-        hi, lo = _split_planes_of(cols)
+        hi, lo = split_planes(cols)
         assert torch.equal(got.hi[:, :B * H * W], hi) and torch.equal(got.lo[:, :B * H * W], lo), f"im2col3x3_t {H}x{W}"
     img = randn(g, B, 3, *geom.cfg["img_size"])
     got = ops.im2col_patch_t(img, geom.cfg["patch"])
     cols = F.unfold(img, geom.cfg["patch"], stride=geom.cfg["patch"])
     cols = cols.permute(1, 0, 2).reshape(cols.shape[1], -1)
-    hi, lo = _split_planes_of(cols)
+    hi, lo = split_planes(cols)
     assert torch.equal(got.hi[:, :cols.shape[1]], hi) and torch.equal(got.lo[:, :cols.shape[1]], lo), "im2col_patch_t"
     # the attention operands: per image [N, 3C] -> [3C, N] (TrainStep._attn_bwd), and [Mp, C] -> [C, Mp]
     N, C = geom.N, geom.C
