@@ -38,6 +38,15 @@ def taskprompter(name):
         "tp_cfg5": dict(tasks=["semseg", "depth", "3ddet"], num_output={"semseg": 19, "depth": 1, "3ddet": 18},
                         img_size=(1024, 2048), patch=16, C=1024, depth=24, heads=16, select=[6, 12, 18],
                         e=300, f=350, chan_nheads=1, use_ctr=False),
+        # the reference's own model configs (TP/configs/nyud/nyud_vitLp16_taskprompter.yml and
+        # TP/configs/pascal/pascal_vitBp16_taskprompter.yml; select from taskprompter.py:675 / :683)
+        "tp_nyud_vitL": dict(tasks=NYUD_TASKS, num_output=NYUD_OUT, img_size=(448, 576), patch=16, C=1024, depth=24,
+                             heads=16, select=[6, 12, 18], e=768, f=768, chan_nheads=16, use_ctr=False),
+        "tp_pascal_vitB": dict(tasks=PASCAL_TASKS, num_output=PASCAL_OUT, img_size=(512, 512), patch=16, C=768,
+                               depth=12, heads=12, select=[3, 6, 9], e=780, f=1024, chan_nheads=16, use_ctr=True),
+        # a 4-block slice of tp_pascal_vitB (4 x 4 channel windows with ctr, e = 780, f = 1024) for the reverse pass
+        "tp_pascal_vitB_d4": dict(tasks=PASCAL_TASKS, num_output=PASCAL_OUT, img_size=(512, 512), patch=16, C=768,
+                                  depth=4, heads=12, select=[1, 2, 3], e=780, f=1024, chan_nheads=16, use_ctr=True),
         # long, non-square sequence (N = 2 + 16*128 = 2050 tokens) at ViT-L width: cheap stand-in for cfg5 in tests
         "tp_long": dict(tasks=["semseg", "depth"], num_output={"semseg": 19, "depth": 1},
                         img_size=(256, 2048), patch=16, C=1024, depth=4, heads=16, select=[1, 2, 3],
@@ -114,6 +123,9 @@ def invpt(name):
         # BASELINE.json configs[2]: InvPT ViT-L PASCAL-Context
         "ip_cfg3": dict(tasks=PASCAL_TASKS, num_output=PASCAL_OUT, img_size=(512, 512), patch=16, C=1024,
                         depth=24, heads=16, select=[6, 12, 18], embed_dim=512, pred_const=64, down=2),
+        # the reference's NYUD model (IP/configs/nyud/nyud_vitLp16.yml; select from IP vit.py:560)
+        "ip_nyud_vitL": dict(tasks=NYUD_TASKS, num_output=NYUD_OUT, img_size=(448, 576), patch=16, C=1024,
+                             depth=24, heads=16, select=[6, 12, 18], embed_dim=512, pred_const=64, down=2),
     }[name]
     c = dict(c)
     c["name"] = name

@@ -1,4 +1,5 @@
-"""What the benched plans launch: their geometries, the key of each recorded ops call, and the recorder.
+"""What the plans launch: the runs the float64 suites cover (RUNS), their geometries, the key of each recorded ops
+call, and the recorder.
 
 A plan test runs a forward with pass-through recorders around some ops functions (recording) and turns each call into a
 hashable key, so the calls can be compared with a table derived from the config (glue_key) or replayed on fresh buffers
@@ -18,16 +19,71 @@ def frozen(d):
     return tuple(sorted(d.items()))
 
 
+# ---- the runs -------------------------------------------------------------------------------------------------------------
+def bench_batch(name):
+    import bench
+    return bench.DEFAULT_BATCH[name]
+
+
+BENCHED = ["tp_cfg4", "tp_cfg2", "tp_cfg5", "ip_cfg3", "tps_swinB"]
+VAL_BATCH = 6            # valBatch of every ViT yml of the reference (TP/configs/**, IP/configs/**)
+LAST_PASCAL_BATCH = 5    # the ragged last validation batch of PASCAL-Context: 5105 images = 850 x 6 + 5
+TR_BATCH = 2             # trBatch of the same ymls
+SWIN_VAL_BATCH = 4       # valBatch of cs_swinB_taskprompter.yml
+
+
+def _runs():
+    """(config, batch, mode) of every run the float64 suites cover. mode: "forward" (model(x); for a Swin model also
+    model.backbone(x)), "predict" (model.predict(x)) or "train" (one TrainStep forward and reverse pass). The bench
+    configs at the bench batch; the reference's own model configs (and those of tp_cfg4 = pascal_vitLp16_taskprompter,
+    ip_cfg3 = InvPT pascal_vitLp16, tps_swinB3d = cs_swinB_taskprompter) at its validation and training batches: the
+    batch sets every GEMM's row count, its tile count and stream-K split, and the trip counts of the glue kernels."""
+    runs = []
+    for name in BENCHED:
+        # a ViT TaskPrompter with the '3ddet' task has no predict(): get_output is not defined for '3ddet' (plans.py)
+        vit_det = name.startswith("tp_") and "3ddet" in configs.taskprompter(name)["tasks"]
+        modes = ("forward",) if vit_det else ("forward", "predict")
+        runs += [(name, bench_batch(name), m) for m in modes]
+    runs += [("tps_swinB3d", 1, m) for m in ("forward", "predict")]
+    runs += [(name, 4, "train") for name in ("tp_cfg4", "tp_cfg2")]
+    for name in ("tp_nyud_vitL", "tp_pascal_vitB", "ip_nyud_vitL", "tp_cfg4", "ip_cfg3"):
+        runs += [(name, VAL_BATCH, m) for m in ("forward", "predict")]
+    for name in ("tp_cfg4", "tp_pascal_vitB", "ip_cfg3"):
+        runs += [(name, LAST_PASCAL_BATCH, m) for m in ("forward", "predict")]
+    runs.append(("tps_swinB3d", SWIN_VAL_BATCH, "predict"))
+    runs += [(name, TR_BATCH, "train") for name in ("tp_cfg4", "tp_pascal_vitB", "tp_nyud_vitL")]
+    assert len(set(runs)) == len(runs)
+    return runs
+
+
+RUNS = _runs()
+# the batch each config was first tested at: its runs there keep the config name alone as their test id
+_FIRST_BATCH = {"tp_cfg4": 4, "tp_cfg2": 4, "tp_cfg5": 1, "ip_cfg3": 4, "tps_swinB": 1, "tps_swinB3d": 1}
+
+
+def run_id(name, B):
+    """The test id of a run: the config and the batch (tp_pascal_vitB-b6); the config alone at its first batch."""
+    return name if _FIRST_BATCH.get(name) == B else f"{name}-b{B}"
+
+
+def runs(modes, family=None):
+    """The distinct (config, batch) of the runs in `modes`, in RUNS order; family: the config name prefix ("tp_", "ip_",
+    "tps_") or a tuple of them."""
+    out = []
+    for name, B, m in RUNS:
+        if m in modes and (family is None or name.startswith(family)) and (name, B) not in out:
+            out.append((name, B))
+    return out
+
+
 # ---- geometry ------------------------------------------------------------------------------------------------------------
 class TPGeom:
-    """A benched TaskPrompter (ViT) forward or training step at its bench batch (bench.DEFAULT_BATCH)."""
+    """A TaskPrompter (ViT) forward or training step at batch B (default: the bench batch, bench.DEFAULT_BATCH)."""
 
-    def __init__(self, name):
-        import bench
-
+    def __init__(self, name, B=None):
         cfg = configs.taskprompter(name)
         self.name, self.cfg = name, cfg
-        self.B = bench.DEFAULT_BATCH[name]
+        self.B = bench_batch(name) if B is None else B
         self.tasks, self.T = list(cfg["tasks"]), len(cfg["tasks"])
         self.img = tuple(cfg["img_size"])
         self.patch = cfg["patch"]
@@ -38,7 +94,7 @@ class TPGeom:
         self.dh = self.C // self.H
         self.nh = self.nw = int(round(math.sqrt(cfg["chan_nheads"])))
         self.e, self.f = cfg["e"], cfg["f"]
-        self.f_ld = round_up(self.f, 8)
+        self.e_ld, self.f_ld = round_up(self.e, 8), round_up(self.f, 8)
         self.use_ctr = cfg["use_ctr"]
         self.h4, self.w4 = 4 * self.gh, 4 * self.gw      # ConvHead: predictions at 4x the token grid
         self.M4 = self.B * self.h4 * self.w4             # rows of the heads' mt_proj.1 BatchNorm
@@ -48,14 +104,12 @@ class TPGeom:
 
 
 class IPGeom:
-    """The benched InvPT forward at its bench batch (invpt.py _Plan)."""
+    """An InvPT forward at batch B (default: the bench batch) (invpt.py _Plan)."""
 
-    def __init__(self, name):
-        import bench
-
+    def __init__(self, name, B=None):
         cfg = configs.invpt(name)
         self.name, self.cfg = name, cfg
-        self.B = bench.DEFAULT_BATCH[name]
+        self.B = bench_batch(name) if B is None else B
         self.tasks, self.T = list(cfg["tasks"]), len(cfg["tasks"])
         self.img = tuple(cfg["img_size"])
         self.patch = cfg["patch"]

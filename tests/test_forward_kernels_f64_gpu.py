@@ -1,6 +1,8 @@
 """-m gpu: the forward glue kernels (csrc/prompting.cu, csrc/invpt.cu, csrc/rowwise.cu) at the geometries the benched
-forwards really run -- tp_cfg4, tp_cfg2, tp_cfg5 and ip_cfg3 at bench.DEFAULT_BATCH -- against float64 references
-written from each operation's definition (F.interpolate, F.conv2d(groups=C), F.avg_pool2d(ceil_mode=True),
+forwards and predict() really run -- the TaskPrompter and InvPT runs of plan_calls.RUNS: tp_cfg4, tp_cfg2, tp_cfg5 and
+ip_cfg3 at bench.DEFAULT_BATCH, the reference's own model configs (tp_nyud_vitL, tp_pascal_vitB, ip_nyud_vitL) and
+tp_cfg4 / ip_cfg3 at the reference's validation batch 6, and the PASCAL ones at the ragged last validation batch 5 --
+against float64 references written from each operation's definition (F.interpolate, F.conv2d(groups=C), F.avg_pool2d(ceil_mode=True),
 F.layer_norm, softmax, the windowed sums, exact-erf GELU), element by element.
 
 Error model: tests/f64_checks.py. Every assert names the bound it uses.
@@ -12,8 +14,9 @@ ratio whose fp32 coordinates are inexact).
 Around every output the test fills a sentinel (padding columns up to ld, guard rows before and after, the other
 tasks' slices of a joint buffer, a second plane where there is one plane); after the call it must be bit-identical.
 
-The geometry table (TABLE) is derived from oracle/configs.py and bench.DEFAULT_BATCH; test_plans_call_only_tabled_shapes
-runs each benched plan once and fails when a plan calls a glue kernel at a shape the table does not hold."""
+The geometry table (TABLE) is derived from oracle/configs.py and each run's batch; test_plans_call_only_tabled_shapes
+runs each plan's forward and predict() once and fails when a plan calls a glue kernel at a shape the table does not
+hold."""
 import math
 
 import pytest
@@ -24,10 +27,10 @@ from f64_checks import (LAM, U, Guarded, assert_planes_bit_exact, check, check_p
                         ops, randn, report, round_up, split_bound, sum_tol)  # noqa: F401
 from kernel_cases import (E_BIL, bilinear_case, gate_case, layernorm_case, ln_bound, ln_input, postproc_case,
                           ref_bilinear, ref_gates, ref_im2col, ref_layernorm, ref_postproc, rows_of)
-from plan_calls import IPGeom, TPGeom, bil, frozen, glue_key, recording
+from plan_calls import RUNS as ALL_RUNS, IPGeom, TPGeom, bil, frozen, glue_key, recording, run_id, runs
 
 pytestmark = [pytest.mark.timeout(1200)]      # the GPU tests are marked one by one: the CPU self-checks are not
-BENCHED = ["tp_cfg4", "tp_cfg2", "tp_cfg5", "ip_cfg3"]
+RUNS = runs(("forward", "predict"), ("tp_", "ip_"))        # (config, batch)
 
 
 def assert_pow2_ratio(src, dst):
@@ -39,8 +42,8 @@ def assert_pow2_ratio(src, dst):
 
 
 # ---- geometry ----------------------------------------------------------------------------------------------------------
-def _geom(name):
-    return IPGeom(name) if name.startswith("ip_") else TPGeom(name)
+def _geom(name, B):
+    return IPGeom(name, B) if name.startswith("ip_") else TPGeom(name, B)
 
 
 def _tp_table(g):
@@ -116,21 +119,23 @@ def _ip_table(g):
 _TABLES = {}
 
 
-def table(name):
-    if name not in _TABLES:
+def table(name, B):
+    if (name, B) not in _TABLES:
         import mtt_b200  # noqa: F401
-        g = _geom(name)
-        _TABLES[name] = (g, _ip_table(g) if name.startswith("ip_") else _tp_table(g))
-    return _TABLES[name]
+        g = _geom(name, B)
+        _TABLES[(name, B)] = (g, _ip_table(g) if name.startswith("ip_") else _tp_table(g))
+    return _TABLES[(name, B)]
+
+
+def _runs_calling(fn):
+    """(config, batch) parameters of the runs that call `fn`."""
+    return [pytest.param(name, B, id=run_id(name, B)) for name, B in RUNS if table(name, B)[1].get(fn)]
 
 
 def _cases(fn):
-    """(config, nsplit) parameters of the configs whose benched forward calls `fn` (a kernel that writes split planes)."""
-    out = []
-    for name in BENCHED:
-        if table(name)[1].get(fn):
-            out += [pytest.param(name, ns, id=f"{name}-ns{ns}") for ns in (2, 1)]
-    return out
+    """(config, batch, nsplit) parameters of the runs that call `fn` (a kernel that writes split planes)."""
+    return [pytest.param(name, B, ns, id=f"{run_id(name, B)}-ns{ns}") for name, B in RUNS if table(name, B)[1].get(fn)
+            for ns in (2, 1)]
 
 
 RECORDED = ["im2col_patch", "broadcast_rows", "layernorm", "chan_logits", "gated_conv1x1", "ctr_weights", "ctr_mix",
@@ -140,30 +145,37 @@ RECORDED = ["im2col_patch", "broadcast_rows", "layernorm", "chan_logits", "gated
 
 @pytest.mark.gpu
 def test_plans_call_only_tabled_shapes(cuda_dev):
-    """Each benched plan at its bench batch runs one forward with pass-through recorders around the ops glue functions:
-    every (function, shape arguments) pair it calls must be in TABLE, so a plan that starts calling a kernel at a new
-    shape fails here instead of leaving the table (and the kernel tests built from it) stale."""
+    """Each plan at each run's batch runs one forward and, where the run list has it, one predict() (evaluation reaches
+    bilinear_postproc only through predict()) with pass-through recorders around the ops glue functions: every
+    (function, shape arguments) pair it calls must be in TABLE, so a plan that starts calling a kernel at a new shape
+    fails here instead of leaving the table (and the kernel tests built from it) stale."""
     import bench
     from mtt_b200 import ops
 
-    for name in BENCHED:
-        g, tab = table(name)
+    for name, B in RUNS:
+        g, tab = table(name, B)
         cfg, M, _ = bench.family(name)
         torch.manual_seed(0)
-        with recording(ops, RECORDED, glue_key, []) as seen:
-            with torch.device(cuda_dev):
-                model = M.build_from_config(cfg, nsplit=2, use_graph=False).eval()
-            with torch.no_grad():
-                model(torch.randn(g.B, 3, *cfg["img_size"], device=cuda_dev))
-        torch.cuda.synchronize()
-        del model
-        torch.cuda.empty_cache()
+        with torch.device(cuda_dev):
+            model = M.build_from_config(cfg, nsplit=2, use_graph=False).eval()
+        x = torch.randn(g.B, 3, *cfg["img_size"], device=cuda_dev)
         want = {(fn, frozen(d)) for fn, ds in tab.items() for d in ds}
-        got = {(fn, frozen(d)) for fn, d in seen}
-        assert got, f"{name}: no glue call recorded"
-        missing = sorted(got - want, key=str)
-        assert not missing, f"{name}: the plan calls glue kernels at shapes the table does not hold: {missing[:6]}"
-        print(f"{name}: {len(got)} distinct glue calls, all in the table ({len(want)} tabled)")
+        for mode in [m for n, b, m in ALL_RUNS if (n, b) == (name, B)]:
+            with recording(ops, RECORDED, glue_key, []) as seen:
+                with torch.no_grad():
+                    model(x) if mode == "forward" else model.predict(x)
+            torch.cuda.synchronize()
+            got = {(fn, frozen(d)) for fn, d in seen}
+            assert got, f"{name} b{B} {mode}: no glue call recorded"
+            missing = sorted(got - want, key=str)
+            assert not missing, f"{name} b{B} {mode}: the plan calls glue kernels at shapes the table does not " \
+                                f"hold: {missing[:6]}"
+            if mode == "predict":
+                assert "bilinear_postproc" in {fn for fn, _ in got}, f"{name} b{B}: predict() made no fused " \
+                                                                      f"post-processing"
+            print(f"{name} b{B} {mode}: {len(got)} distinct glue calls, all in the table ({len(want)} tabled)")
+        del model, x
+        torch.cuda.empty_cache()
 
 
 # ---- float64 references (device-agnostic: the CPU self-check runs them too) -----------------------------------------------
@@ -226,11 +238,11 @@ def ref_fuse(raw, scale, prev, wf, bf, B, T, qh, qw):
 
 
 # ---- data movement: bit-exact ------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name,ns", _cases("im2col_patch"))
+@pytest.mark.parametrize("name,B,ns", _cases("im2col_patch"))
 @pytest.mark.gpu
-def test_im2col_patch(ops, name, ns):
+def test_im2col_patch(ops, name, B, ns):
     """Patch im2col of the whole input batch: planes bit-exact against the split of F.unfold (column order c, ky, kx)."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     for d in tab["im2col_patch"]:
         img = randn(gen(1), *d["shape"])
         rows = d["shape"][0] * g.P
@@ -241,12 +253,12 @@ def test_im2col_patch(ops, name, ns):
         assert_planes_bit_exact(sp, ref_im2col(img, d["patch"]), "im2col_patch")
 
 
-@pytest.mark.parametrize("name", BENCHED)
+@pytest.mark.parametrize("name,B", _runs_calling("broadcast_rows"))
 @pytest.mark.gpu
-def test_broadcast_rows_and_nhwc_to_nchw(ops, name):
+def test_broadcast_rows_and_nhwc_to_nchw(ops, name, B):
     """Prompt / cls rows broadcast into every image's group of the joint stream (the patch rows stay as they were), and
     the 3ddet map's NHWC -> NCHW copy: bit-exact."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     for d in tab["broadcast_rows"]:
         src = randn(gen(2), d["T"], d["C"])
         gb = Guarded((d["B"] * d["group_rows"], d["ld"]), torch.float32)
@@ -265,12 +277,12 @@ def test_broadcast_rows_and_nhwc_to_nchw(ops, name):
         assert torch.equal(gb.view, x[:, :d["Cd"]].reshape(d["B"], d["H"], d["W"], d["Cd"]).permute(0, 3, 1, 2))
 
 
-@pytest.mark.parametrize("name,ns", _cases("zero_insert"))
+@pytest.mark.parametrize("name,B,ns", _cases("zero_insert"))
 @pytest.mark.gpu
-def test_zero_insert_and_split_rows(ops, name, ns):
+def test_zero_insert_and_split_rows(ops, name, B, ns):
     """InvPT's scale_embed inputs from the patch rows of the joint stream (row 0 of each image is the cls token):
     zero insertion for the transposed conv and the plain row gather, planes bit-exact."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     for d in tab["zero_insert"]:
         B, h, w, C = d["B"], d["h"], d["w"], d["Cdim"]
         x = randn(gen(5), B * d["src_group"], d["ld_in"])
@@ -294,21 +306,21 @@ def test_zero_insert_and_split_rows(ops, name, ns):
 
 
 # ---- LayerNorm ------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name", [n for n in BENCHED if table(n)[1].get("layernorm")])
+@pytest.mark.parametrize("name,B", _runs_calling("layernorm"))
 @pytest.mark.gpu
-def test_layernorm(ops, name):
+def test_layernorm(ops, name, B):
     """mtt_layernorm at the plans' rows x widths: TaskPrompter's final norm (C = 1024 / 768: the register path) and
     InvPT's per-stage norm1 (C = 576 / 288 / 144, up to 81920 rows: the general path), fp32 out with ld = C."""
-    g, tab = table(name)
-    report(f"layernorm {name}", [layernorm_case(ops, d, 10 + i) for i, d in enumerate(tab["layernorm"])])
+    g, tab = table(name, B)
+    report(f"layernorm {name} b{B}", [layernorm_case(ops, d, 10 + i) for i, d in enumerate(tab["layernorm"])])
 
 
-@pytest.mark.parametrize("name,ns", _cases("layernorm_seg"))
+@pytest.mark.parametrize("name,B,ns", _cases("layernorm_seg"))
 @pytest.mark.gpu
-def test_layernorm_seg(ops, name, ns):
+def test_layernorm_seg(ops, name, B, ns):
     """ViT final norm over the gathered patch rows (S = 1) and InvPT's joint-channel norm over all T tasks' slices
     (S = T segments, statistics over T * C values) with the per-task output rows; fp32 or split out as the plan has it."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     ratios = []
     for i, d in enumerate(tab["layernorm_seg"]):
         rows, cols, S = d["rows"], d["cols"], d["S"]
@@ -347,17 +359,17 @@ def test_layernorm_seg(ops, name, ns):
             ratios.append(check(v, want, e + split_bound(ns, want.abs() + e),
                                 f"layernorm_seg S={S} {rows}x{cols} split ns={ns} (LN bound + split bound)"))
     if ratios:
-        report(f"layernorm_seg {name} ns={ns}", ratios)
+        report(f"layernorm_seg {name} b{B} ns={ns}", ratios)
 
 
 # ---- channel-prompt logits, gating, cross-task reweighting ---------------------------------------------------------------------
-@pytest.mark.parametrize("name,ns", _cases("chan_logits"))
+@pytest.mark.parametrize("name,B,ns", _cases("chan_logits"))
 @pytest.mark.gpu
-def test_chan_logits(ops, name, ns):
+def test_chan_logits(ops, name, B, ns):
     """Rc[b,t,c,window] = sum over the window's pixels of cp[b,t,pix] xn[b,T+pix,c], xn as LN1's split planes (one or
     two): 1 window of 32 x 32 (tp_cfg4), 4 x 4 windows of 7 x 9 (tp_cfg2), one 64 x 128 window whose cp slice needs
     ~111 KB of dynamic shared memory (tp_cfg5)."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     for d in tab["chan_logits"]:
         B, N, T, C, gh, gw, nh, nw = (d[k] for k in ("B", "N", "T", "C", "gh", "gw", "nh", "nw"))
         P = gh * gw
@@ -377,27 +389,27 @@ def test_chan_logits(ops, name, ns):
         wp = (gh // nh) * (gw // nw)
         D = math.ceil(wp / 32) + 32                # serial fma over the block's pixel group, then 32 partials in order
         r = check(gb.view, want, sum_tol(D, absum), f"chan_logits {name} (sum_tol D={D})")
-        report(f"chan_logits {name} ns={ns}", [r])
+        report(f"chan_logits {name} b{B} ns={ns}", [r])
 
 
-@pytest.mark.parametrize("name,ns", _cases("gate_split"))
+@pytest.mark.parametrize("name,B,ns", _cases("gate_split"))
 @pytest.mark.gpu
-def test_gate_split(ops, name, ns):
+def test_gate_split(ops, name, B, ns):
     """Spatial and channel gating of all T tasks in one launch, X = the patch rows of the joint stream (x rows offset by
     T inside groups of N), written task after task into the gated-conv workspace layout (task_stride); the slack of
     each 256-byte aligned plane set and the space after the last task stay untouched."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     for d in tab["gate_split"]:
-        report(f"gate_split {name} ns={ns}", gate_case(ops, d, ns, name))
+        report(f"gate_split {name} b{B} ns={ns}", gate_case(ops, d, ns, f"{name} b{B}"))
 
 
-@pytest.mark.parametrize("name", [n for n in BENCHED if table(n)[1].get("ctr_mix")])
+@pytest.mark.parametrize("name,B", _runs_calling("ctr_mix"))
 @pytest.mark.gpu
-def test_ctr_weights_and_mix(ops, name):
+def test_ctr_weights_and_mix(ops, name, B):
     """Cross-task reweighting: w[b,t,j] = W2_t . gelu(W0_t R[b,:,t,j] + b0_t) + b2_t over H heads, then
     acc[t] (+)= sum_j w[b,t,j] F[j] over all ld columns (the header: C = ld, the padding columns carry 0 + 0 and are
     checked like the rest), accumulate off then on."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     d = tab["ctr_weights"][0]
     B, H, T, N = d["B"], d["H"], d["T"], d["N"]
     gg = gen(50)
@@ -434,31 +446,31 @@ def test_ctr_weights_and_mix(ops, name):
         absum = ref_ctr_mix(Fm.double().abs(), Wd.abs(), rpb) + acc0.double().abs()
         ratios.append(check(ga.view, want, (T + 1) * U * absum, f"ctr_mix {name} acc={d['accumulate']} ((T+1)u)"))
         assert (ga.view[..., g.f:] == 0).all(), "ctr_mix padding columns: sum of w x 0"
-    report(f"ctr {name}", ratios)
+    report(f"ctr {name} b{B}", ratios)
 
 
 # ---- bilinear ----------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name,ns", _cases("bilinear"))
+@pytest.mark.parametrize("name,B,ns", _cases("bilinear"))
 @pytest.mark.gpu
-def test_bilinear(ops, name, ns):
+def test_bilinear(ops, name, B, ns):
     """Every bilinear resize the plan runs, in its form: NHWC split (both planes, even C, no fp32 out: the FAST form; one
     plane: the vectorised general form) for the decoder's x4 up-sampling (C = 350 / 768, two pairs per lane, a partial
     last chunk), InvPT's 32 -> 16 downsample of the final tokens and its UpEmbed x2 with in_row_offset; NHWC fp32
     accumulate with in / out row offsets (InvPT's attention output into each task's slice); NCHW to the image size."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     ratios = [bilinear_case(ops, d, ns, 60 + i) for i, d in enumerate(tab["bilinear"])
               if d["form"] == "split" or ns == 2]
     if ratios:
-        report(f"bilinear {name} ns={ns}", ratios)
+        report(f"bilinear {name} b{B} ns={ns}", ratios)
 
 
-@pytest.mark.parametrize("name,ns", _cases("bilinear_sum3"))
+@pytest.mark.parametrize("name,B,ns", _cases("bilinear_sum3"))
 @pytest.mark.gpu
-def test_bilinear_sum3(ops, name, ns):
+def test_bilinear_sum3(ops, name, B, ns):
     """InvPT's multi-scale aggregation: the three stages' maps (16², 32², 64², the first one a task's slice of the joint
     LayerNorm output) resized to 128 x 128 and summed, written once as split planes (C = 576: 5 chunks of 128 channels,
     half the pairs of the last one idle)."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     ratios = []
     for i, d in enumerate(tab["bilinear_sum3"]):
         B, C, H2, W2 = d["B"], d["Cdim"], d["H2"], d["W2"]
@@ -476,30 +488,30 @@ def test_bilinear_sum3(ops, name, ns):
         wn, an = want.permute(0, 2, 3, 1).reshape(-1, C), absr.permute(0, 2, 3, 1).reshape(-1, C)
         e = (E_BIL + 2 * U) * an                                     # each source's resize, then two more sums
         ratios.append(check_planes(sp, wn, e, f"bilinear_sum3 slice {i} (6u per source + 2u)"))
-    report(f"bilinear_sum3 {name} ns={ns}", ratios)
+    report(f"bilinear_sum3 {name} b{B} ns={ns}", ratios)
 
 
-@pytest.mark.parametrize("name", [n for n in BENCHED if table(n)[1].get("bilinear_postproc")])
+@pytest.mark.parametrize("name,B", _runs_calling("bilinear_postproc"))
 @pytest.mark.gpu
-def test_bilinear_postproc(ops, name):
+def test_bilinear_postproc(ops, name, B):
     """The final resize fused with get_output at full output size, for each task's kind: argmax over 21 / 7 / 40 / 19
     classes, 255 sigmoid, 255 softmax[1], normalised normals, clamped depth. A class must be exact wherever the float64
     top-2 margin exceeds twice the value bound, and one of the tied classes elsewhere."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     ratios = [postproc_case(ops, d, 120 + i) for i, d in enumerate(tab["bilinear_postproc"])]
     ratios = [r for r in ratios if r is not None]
     if ratios:
-        report(f"bilinear_postproc {name}", ratios)
+        report(f"bilinear_postproc {name} b{B}", ratios)
 
 
 # ---- InvPT token reductions and cross-task attention softmax -------------------------------------------------------------------
-@pytest.mark.parametrize("name,ns", _cases("dwconv3x3_s2"))
+@pytest.mark.parametrize("name,B,ns", _cases("dwconv3x3_s2"))
 @pytest.mark.gpu
-def test_dwconv_and_avgpool(ops, name, ns):
+def test_dwconv_and_avgpool(ops, name, B, ns):
     """Per-stage Q and KV token reductions at C = 576 / 288 / 144 (256-, 256- and 128-thread blocks, ragged channel
     loops): per-task depthwise 3x3 stride-2 conv (bias + 9 fma) against F.conv2d(groups=C), and the s x s average pool
     (s = 2 / 4 / 8) against F.avg_pool2d(ceil_mode=True)."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     ratios = []
     for i, d in enumerate(tab["dwconv3x3_s2"]):
         B, T, h, w, C = d["B"], d["T"], d["h"], d["w"], d["Cdim"]
@@ -524,16 +536,16 @@ def test_dwconv_and_avgpool(ops, name, ns):
         # a serial sum of s * s terms, then the product with 1 / count (a power of two here: exact)
         ratios.append(check_planes(sp, want, sum_tol(s * s, absr) + U * want.abs(),
                                    f"avgpool {h}x{w} s={s} C={C} (sum_tol D=s^2 + u)"))
-    report(f"dwconv/avgpool {name} ns={ns}", ratios)
+    report(f"dwconv/avgpool {name} b{B} ns={ns}", ratios)
 
 
-@pytest.mark.parametrize("name,ns", _cases("invpt_fuse_softmax"))
+@pytest.mark.parametrize("name,B,ns", _cases("invpt_fuse_softmax"))
 @pytest.mark.gpu
-def test_invpt_fuse_softmax(ops, name, ns):
+def test_invpt_fuse_softmax(ops, name, B, ns):
     """The step between InvPT's two attention GEMMs at every stage: Tk = 320 keys (10 per lane), Lq = 320 / 1280 / 5120
     queries, cross-scale fusion with the previous stage's fused score (x2 bilinear per task over the query grid) at stages
     1 and 2, the fused score written in place of the raw one (stages 0 and 1), P = softmax as split rows."""
-    g, tab = table(name)
+    g, tab = table(name, B)
     ratios = []
     prev = None
     for i, d in enumerate(tab["invpt_fuse_softmax"]):
@@ -578,7 +590,7 @@ def test_invpt_fuse_softmax(ops, name, ns):
         ratios.append(check_planes(sp, Pw.reshape(B * 2 * Lq, Tk), e_P.reshape(B * 2 * Lq, Tk),
                                    f"softmax P stage {i} (perturbation + expf + sum_tol D={D})"))
         prev = score if d["score_out"] else None
-    report(f"invpt_fuse_softmax {name} ns={ns}", ratios)
+    report(f"invpt_fuse_softmax {name} b{B} ns={ns}", ratios)
 
 
 # ---- CPU self-check of the references ----------------------------------------------------------------------------------------
@@ -680,15 +692,41 @@ def test_references_against_the_torch_restatement(monkeypatch):
 
 
 def test_geometry_table_is_derived_for_every_benched_config():
-    """The table derives for every benched config, holds only power-of-two resizes, and reaches the shapes the kernel
-    tests are about (the 64 x 128 channel window, Tk = 320 at every InvPT stage)."""
-    for name in BENCHED:
-        g, tab = table(name)
-        for d in tab["bilinear"]:
+    """The table derives for every run, holds only power-of-two resizes, and reaches the shapes the kernel tests are
+    about: the 64 x 128 channel window, Tk = 320 at every ip_cfg3 stage; at the reference's own configs Tk = 252 at every
+    ip_nyud_vitL stage (a ragged last lane of the softmax and a K tail of the grouped P.V GEMM), the 784-wide e and
+    1024-wide f of tp_pascal_vitB with ctr over 4 x 4 channel windows at H = 12, N = 1012 tokens at 16 heads
+    (tp_nyud_vitL), and M = 6 * 1029 rows at valBatch 6."""
+    for name, B in RUNS:
+        g, tab = table(name, B)
+        assert g.B == B
+        for d in tab["bilinear"] + tab.get("bilinear_postproc", []):
             assert_pow2_ratio(d["h"], d["H2"])
             assert_pow2_ratio(d["w"], d["W2"])
-        for d in tab.get("bilinear_postproc", []):
-            assert_pow2_ratio(d["h"], d["H2"])
-            assert_pow2_ratio(d["w"], d["W2"])
-    assert table("tp_cfg5")[1]["chan_logits"][0]["gh"] * table("tp_cfg5")[1]["chan_logits"][0]["gw"] == 8192
-    assert [d["Tk"] for d in table("ip_cfg3")[1]["invpt_fuse_softmax"]] == [320, 320, 320]
+        for d in tab.get("bilinear_sum3", []):
+            for h, w, *_ in d["srcs"]:
+                assert_pow2_ratio(h, d["H2"])
+                assert_pow2_ratio(w, d["W2"])
+    assert {(n, B) for n, B in RUNS} >= {(n, 6) for n in ("tp_nyud_vitL", "tp_pascal_vitB", "ip_nyud_vitL", "tp_cfg4",
+                                                         "ip_cfg3")} | {(n, 5) for n in ("tp_cfg4", "tp_pascal_vitB",
+                                                                                          "ip_cfg3")}
+    cl5 = table("tp_cfg5", 1)[1]["chan_logits"][0]
+    assert cl5["gh"] * cl5["gw"] == 8192
+    assert [d["Tk"] for d in table("ip_cfg3", 4)[1]["invpt_fuse_softmax"]] == [320, 320, 320]
+    g, tab = table("ip_nyud_vitL", 6)
+    assert [d["Tk"] for d in tab["invpt_fuse_softmax"]] == [252, 252, 252]
+    assert [d["ldp"] for d in tab["invpt_fuse_softmax"]] == [256, 256, 256]
+    assert [d["Lq"] for d in tab["invpt_fuse_softmax"]] == [252, 1008, 4032]
+    assert [s["Tk"] % 64 for s in g.stages] == [60, 60, 60]            # P.V's K = Tk: a 60-deep last K-stage
+    assert {(d["H2"], d["W2"]) for d in tab["bilinear_sum3"]} == {(112, 144)}
+    g, tab = table("tp_pascal_vitB", 6)
+    assert (g.e, g.e_ld, g.f, g.f_ld) == (780, 784, 1024, 1024)
+    assert tab["ctr_weights"] == [dict(B=6, H=12, T=5, N=1029)]
+    assert (tab["chan_logits"][0]["nh"], tab["chan_logits"][0]["nw"], tab["chan_logits"][0]["C"]) == (4, 4, 768)
+    assert bil(1024, 6, 32, 32, 1024, 128, 128, "split", ld_out=1024) in tab["bilinear"]
+    assert tab["layernorm"][0]["rows"] == 6 * 1029 == table("tp_cfg4", 6)[1]["layernorm"][0]["rows"]
+    g, tab = table("tp_nyud_vitL", 6)
+    gs = tab["gate_split"][0]
+    assert (gs["N"], gs["H"], gs["C"], gs["nh"], gs["nw"], gs["gh"] // gs["nh"], gs["gw"] // gs["nw"]) == \
+        (1012, 16, 1024, 4, 4, 7, 9)
+    assert table("tp_pascal_vitB", 5)[1]["layernorm"][0]["rows"] == 5 * 1029

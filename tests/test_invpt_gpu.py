@@ -7,9 +7,9 @@ import os
 import pytest
 import torch
 
+from model_checks import check_parity as _check
 from oracle import configs
 from oracle import invpt_ref as IPR
-from test_taskprompter_gpu import _check
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")

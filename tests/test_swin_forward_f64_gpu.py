@@ -1,6 +1,7 @@
-"""The non-tensor-core kernels of the Swin TaskPrompter forward at every geometry the plans launch -- tps_swinB (two tasks)
-and tps_swinB3d (three tasks with '3ddet', nn.Identity as its detection head) at batch 1, in the wrapper forward
-("full"), predict() ("postproc") and the backbone forward -- against float64, element by element.
+"""The non-tensor-core kernels of the Swin TaskPrompter forward at every geometry the plans launch -- the Swin runs of
+plan_calls.RUNS: tps_swinB (two tasks) and tps_swinB3d (three tasks with '3ddet', nn.Identity as its detection head) at
+batch 1 in the wrapper forward ("full"), predict() ("postproc") and the backbone forward, and tps_swinB3d's predict() at
+the reference's validation batch 4 -- against float64, element by element.
 
 Geometry. SwinGeom derives, from the config alone, the stage maps (C, heads, window 12, shift 0 / 6, nW, T), the
 decoder levels (maps, f) and the head and output sizes; swin_table turns it into the list of calls each mode makes
@@ -29,11 +30,17 @@ from kernel_cases import (E_BIL, attention_case, bilinear_case, chan_attention_c
                           fp32_coords_exact, gate_case, gather_scatter_case, layernorm_case, nan_split,
                           assert_untouched, postproc_case, ref_bilinear, ref_bilinear_any, ref_im2col, rows_of)
 from oracle import configs
-from plan_calls import DET, SwinGeom, bil, frozen, glue_key, recording
+from plan_calls import DET, RUNS, SwinGeom, bil, frozen, glue_key, recording, run_id
 
 pytestmark = [pytest.mark.timeout(1200)]      # the GPU tests are marked one by one: the CPU checks are not
-CONFIGS = ["tps_swinB", "tps_swinB3d"]
 MODES = ["full", "postproc", "backbone"]
+_MODES_OF = {"forward": ["full", "backbone"], "predict": ["postproc"]}
+# {(config, batch): the modes its runs make}, in RUNS order
+SWIN_RUNS = {}
+for _n, _B, _m in RUNS:
+    if _n.startswith("tps_"):
+        SWIN_RUNS.setdefault((_n, _B), [])
+        SWIN_RUNS[(_n, _B)] = [m for m in MODES if m in SWIN_RUNS[(_n, _B)] + _MODES_OF[_m]]
 RECORDED = ["layernorm", "split_f32", "im2col_patch", "broadcast_rows", "swin_window_gather", "swin_window_attention",
             "swin_window_scatter", "transpose_split", "swin_chan_attention", "swin_merge_gather", "conv3x3_s2_maps",
             "swin_chan_up", "gated_conv1x1", "bilinear", "bilinear_postproc", "nhwc_to_nchw"]
@@ -104,31 +111,31 @@ def swin_table(g, mode):
 _GEOMS = {}
 
 
-def geom(name):
-    if name not in _GEOMS:
-        _GEOMS[name] = SwinGeom(name)
-    return _GEOMS[name]
+def geom(name, B=1):
+    if (name, B) not in _GEOMS:
+        _GEOMS[(name, B)] = SwinGeom(name, B)
+    return _GEOMS[(name, B)]
 
 
-def table(name):
-    """Every call of the three modes of `name`, merged."""
+def table(name, B=1):
+    """Every call of the modes the runs of `name` at batch B make, merged."""
     out = {}
-    for mode in MODES:
-        for fn, ds in swin_table(geom(name), mode).items():
+    for mode in SWIN_RUNS[(name, B)]:
+        for fn, ds in swin_table(geom(name, B), mode).items():
             out.setdefault(fn, [])
             out[fn] += [d for d in ds if d not in out[fn]]
     return out
 
 
 def entries(fn, split=True):
-    """pytest parameters (config, entry index, nsplit) of every table entry of `fn`; nsplit 1 too where the entry
-    writes split planes (split: True, False, or a predicate of the entry)."""
+    """pytest parameters (config, batch, entry index, nsplit) of every table entry of `fn`; nsplit 1 too where the
+    entry writes split planes (split: True, False, or a predicate of the entry)."""
     out = []
-    for name in CONFIGS:
-        for i, d in enumerate(table(name).get(fn, [])):
+    for name, B in SWIN_RUNS:
+        for i, d in enumerate(table(name, B).get(fn, [])):
             planes = split(d) if callable(split) else split
             for ns in ((2, 1) if planes else (2,)):
-                out.append(pytest.param(name, i, ns, id=f"{name}-{i}-ns{ns}"))
+                out.append(pytest.param(name, B, i, ns, id=f"{run_id(name, B)}-{i}-ns{ns}"))
     return out
 
 
@@ -176,23 +183,24 @@ def assert_same_keys(got, want, what):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", CONFIGS)
-def test_plans_call_exactly_the_tabled_shapes(cuda_dev, name):
-    """One eager pass of each mode at batch 1, parity build: recorded keys == table; a speed-mode build of the wrapper
-    forward records the same keys (the keys hold no plane count)."""
+@pytest.mark.parametrize("name,B", [pytest.param(n, B, id=run_id(n, B)) for n, B in SWIN_RUNS])
+def test_plans_call_exactly_the_tabled_shapes(cuda_dev, name, B):
+    """One eager pass of each mode of the run at its batch, parity build: recorded keys == table; a speed-mode build
+    records the same keys in the first of them (the keys hold no plane count)."""
     import mtt_b200  # noqa: F401
-    g = geom(name)
+    g = geom(name, B)
     x = torch.randn(g.B, 3, *g.img, device=cuda_dev)
     model = build(name, cuda_dev, 2)
-    for mode in MODES:
+    modes = SWIN_RUNS[(name, B)]
+    for mode in modes:
         got = recorded_keys(model, mode, x)
-        assert_same_keys(got, tabled_keys(g, mode), f"{name} {mode}")
-        print(f"{name} {mode}: {len(got)} distinct calls, exactly the table's")
-    par = recorded_keys(model, "full", x)
+        assert_same_keys(got, tabled_keys(g, mode), f"{name} b{B} {mode}")
+        print(f"{name} b{B} {mode}: {len(got)} distinct calls, exactly the table's")
+    par = recorded_keys(model, modes[0], x)
     del model
     torch.cuda.empty_cache()
     model = build(name, cuda_dev, 1)
-    assert recorded_keys(model, "full", x) == par, f"{name}: the speed-mode plan calls other shapes"
+    assert recorded_keys(model, modes[0], x) == par, f"{name} b{B}: the speed-mode plan calls other shapes"
     del model
     torch.cuda.empty_cache()
 
@@ -215,7 +223,9 @@ def test_plans_call_exactly_the_tabled_shapes_emulated(monkeypatch, name):
 
 
 def test_geometry_of_the_swinB_models():
-    """The table reaches the shapes the kernel tests are about."""
+    """The table reaches the shapes the kernel tests are about, at batch 1 and at tps_swinB3d's valBatch 4."""
+    assert list(SWIN_RUNS) == [("tps_swinB", 1), ("tps_swinB3d", 1), ("tps_swinB3d", 4)]
+    assert SWIN_RUNS[("tps_swinB", 1)] == MODES and SWIN_RUNS[("tps_swinB3d", 4)] == ["postproc"]
     for name, T in (("tps_swinB", 2), ("tps_swinB3d", 3)):
         g, tab = geom(name), table(name)
         assert g.T == T and [s["nW"] for s in g.stages] == [512, 128, 32, 8]
@@ -226,6 +236,13 @@ def test_geometry_of_the_swinB_models():
         assert {(d["h"], d["w"], d["H2"], d["W2"]) for d in tab["bilinear_postproc"]} == {(384, 768, 512, 1024)}
     assert len(table("tps_swinB3d")["nhwc_to_nchw"]) == 3 + 1          # 3 distinct level maps (two share 24x48) + fea
     assert not fp32_coords_exact(1024, 768) and fp32_coords_exact(384, 512)
+    tab = table("tps_swinB3d", 4)
+    assert {(d["BW"], d["nW"]) for d in tab["swin_window_attention"]} == {(4 * 512, 512), (4 * 128, 128), (4 * 32, 32),
+                                                                          (4 * 8, 8)}
+    assert {"rows": 4 * 73728, "cols": 128, "ld_in": 128, "f32": True, "split": False} in tab["layernorm"]
+    assert {(d["B"], d["H2"], d["W2"]) for d in tab["bilinear_postproc"]} == {(4, 512, 1024)}
+    assert bil(1, 12, 1024, 2048, 1, 768, 1536, "nchw") in tab["bilinear"]
+    assert len(tab["nhwc_to_nchw"]) == 3                                  # predict(): the 3ddet level maps, no fea
 
 
 # ---- float64: window attention, gather / scatter, channel attention, merging ------------------------------------------------
@@ -234,16 +251,16 @@ def _stage_of(g, C):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("swin_window_attention"))
-def test_window_attention(ops, cuda_dev, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("swin_window_attention"))
+def test_window_attention(ops, cuda_dev, name, B, i, ns):
     """Window attention at each stage x shift of the table (N = T + 144: 146 or 147 rows), all T raw-logit rows."""
-    d = table(name)["swin_window_attention"][i]
-    s = _stage_of(geom(name), d["C"])
+    d = table(name, B)["swin_window_attention"][i]
+    s = _stage_of(geom(name, B), d["C"])
     shift = 6 if d["masked"] else 0
     r = attention_case(ops, cuda_dev, B=d["BW"] // d["nW"], nWy=s["H"] // s["ws"], nWx=s["W"] // s["ws"],
                            ws=s["ws"], shift=shift, T=d["T"], heads=d["heads"], dh=d["C"] // d["heads"],
                            seed=100 * i + d["T"], ns=ns)
-    report(f"window attention {name} C={d['C']} shift={shift} ns={ns} (out, raw logits)", r)
+    report(f"window attention {name} b{B} C={d['C']} shift={shift} ns={ns} (out, raw logits)", r)
     torch.cuda.empty_cache()
 
 
@@ -255,12 +272,12 @@ def _gather_scatter(ops, dev, d, ns, B=None):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("swin_window_scatter"))
-def test_window_gather_and_scatter(ops, cuda_dev, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("swin_window_scatter"))
+def test_window_gather_and_scatter(ops, cuda_dev, name, B, i, ns):
     """Gather (split planes, bit-exact) and scatter (xa, x += xa and the [B, heads, T, T + L] logits map bit-exact,
     the prompt mean within its bound) at each stage x shift x last of the table."""
-    d = table(name)["swin_window_scatter"][i]
-    report(f"window scatter {name} C={d['C']} shift={d['shift']} last={d['last']} (prompt mean)",
+    d = table(name, B)["swin_window_scatter"][i]
+    report(f"window scatter {name} b{B} C={d['C']} shift={d['shift']} last={d['last']} (prompt mean)",
            [_gather_scatter(ops, cuda_dev, d, ns)])
 
 
@@ -275,10 +292,10 @@ def test_window_scatter_grid_stride(ops, cuda_dev, T):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("transpose_split"))
-def test_transpose_split(ops, cuda_dev, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("transpose_split"))
+def test_transpose_split(ops, cuda_dev, name, B, i, ns):
     """[B, L, C] -> split [B*C, L] per stage (L = 73728 ... 1152), NaN pad columns read past C would show: bit-exact."""
-    d = table(name)["transpose_split"][i]
+    d = table(name, B)["transpose_split"][i]
     B, L, C = d["B"], d["L"], d["C"]
     x = padded(B * L, C, cuda_dev)
     x.copy_(randn(gen(200 + i), B * L, C))
@@ -290,19 +307,19 @@ def test_transpose_split(ops, cuda_dev, name, i, ns):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("swin_chan_attention"))
-def test_chan_attention(ops, cuda_dev, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("swin_chan_attention"))
+def test_chan_attention(ops, cuda_dev, name, B, i, ns):
     """Channel attention of the T prompts over the C channels of each stage (C = 128 ... 1024, one 16 x 16 window)."""
-    d = table(name)["swin_chan_attention"][i]
+    d = table(name, B)["swin_chan_attention"][i]
     r = chan_attention_case(ops, cuda_dev, B=d["B"], T=d["T"], C=d["C"], nh=d["nh"], ns=ns)
-    report(f"chan attention {name} T={d['T']} C={d['C']} ns={ns} (raw_chan, chan_out)", r)
+    report(f"chan attention {name} b{B} T={d['T']} C={d['C']} ns={ns} (raw_chan, chan_out)", r)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("swin_merge_gather", split=False))
-def test_merge_gather(ops, cuda_dev, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("swin_merge_gather", split=False))
+def test_merge_gather(ops, cuda_dev, name, B, i, ns):
     """2 x 2 merge (0,0), (1,0), (0,1), (1,1) at each merging stage: bit-exact, pad columns untouched."""
-    d = table(name)["swin_merge_gather"][i]
+    d = table(name, B)["swin_merge_gather"][i]
     B, H, W, C = d["B"], d["H"], d["W"], d["C"]
     x = padded(B * H * W, C, cuda_dev)
     x.copy_(randn(gen(300 + i), B * H * W, C))
@@ -316,13 +333,13 @@ def test_merge_gather(ops, cuda_dev, name, i, ns):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("conv3x3_s2_maps", split=False))
-def test_conv3x3_s2_maps(ops, cuda_dev, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("conv3x3_s2_maps", split=False))
+def test_conv3x3_s2_maps(ops, cuda_dev, name, B, i, ns):
     """spa_attn_ds at each merge: Cin = Cout = heads * T (8 / 16 / 32 at T = 2, 12 / 24 / 48 at T = 3)."""
-    d = table(name)["conv3x3_s2_maps"][i]
+    d = table(name, B)["conv3x3_s2_maps"][i]
     T = d["in_offset"]
     r = conv3x3_s2_case(ops, cuda_dev, B=d["B"], T=T, H=d["H"], W=d["W"], Cin=d["Cin"], seed=400 + i)
-    report(f"conv3x3_s2 {name} Cin={d['Cin']}", [r])
+    report(f"conv3x3_s2 {name} b{B} Cin={d['Cin']}", [r])
 
 
 @pytest.mark.gpu
@@ -335,20 +352,20 @@ def test_conv3x3_s2_maps_grid_stride(ops, cuda_dev):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("swin_chan_up", split=False))
-def test_chan_up(ops, cuda_dev, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("swin_chan_up", split=False))
+def test_chan_up(ops, cuda_dev, name, B, i, ns):
     """process_chan_attn C -> 2C at each merge, B * T rows."""
-    d = table(name)["swin_chan_up"][i]
+    d = table(name, B)["swin_chan_up"][i]
     r = chan_up_case(ops, cuda_dev, BT=d["BT"], C=d["C"], nwin=d["nwin"], seed=500 + i)
-    report(f"chan_up {name} BT={d['BT']} C={d['C']}", [r])
+    report(f"chan_up {name} b{B} BT={d['BT']} C={d['C']}", [r])
 
 
 # ---- float64: stem, LayerNorm, splits, gating, resampling, layout -----------------------------------------------------------
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("im2col_patch"))
-def test_im2col_patch(ops, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("im2col_patch"))
+def test_im2col_patch(ops, name, B, i, ns):
     """Patch 4 on the 768 x 1536 downsampled input: planes bit-exact against the split of F.unfold."""
-    d = table(name)["im2col_patch"][i]
+    d = table(name, B)["im2col_patch"][i]
     img = randn(gen(600), *d["shape"])
     rows = d["shape"][0] * (d["shape"][2] // d["patch"]) * (d["shape"][3] // d["patch"])
     gb, sp, reg = guarded_split(ops, ns, rows, d["ld"], ld=d["ld"])
@@ -359,10 +376,10 @@ def test_im2col_patch(ops, name, i, ns):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("broadcast_rows", split=False))
-def test_broadcast_rows(ops, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("broadcast_rows", split=False))
+def test_broadcast_rows(ops, name, B, i, ns):
     """The T task prompts into each image's prompt rows: bit-exact, nothing else written."""
-    d = table(name)["broadcast_rows"][i]
+    d = table(name, B)["broadcast_rows"][i]
     src = randn(gen(610), d["T"], d["C"])
     gb = Guarded((d["B"] * d["group_rows"], d["ld"]), torch.float32)
     gb.snapshot()
@@ -373,10 +390,10 @@ def test_broadcast_rows(ops, name, i, ns):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("split_f32"))
-def test_split_f32(ops, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("split_f32"))
+def test_split_f32(ops, name, B, i, ns):
     """The prompt rows and the level sum as planes: bit-exact, input pad columns (NaN) not read."""
-    d = table(name)["split_f32"][i]
+    d = table(name, B)["split_f32"][i]
     x = torch.full((d["rows"], d["ld_in"]), float("nan"), device="cuda")[:, :d["cols"]]
     x.copy_(randn(gen(620 + i), d["rows"], d["cols"]))
     gb, sp, reg = guarded_split(ops, ns, d["rows"], d["cols"], ld=d["ld_out"])
@@ -387,52 +404,52 @@ def test_split_f32(ops, name, i, ns):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("layernorm", split=lambda d: d["split"]))
-def test_layernorm(ops, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("layernorm", split=lambda d: d["split"]))
+def test_layernorm(ops, name, B, i, ns):
     """Every LayerNorm: the stage norms over 73 728 x 128 ... 288 x 1024 rows, the prompt rows, the merge norm into
     split planes (4C = 512 ... 4096 columns), the final norm."""
-    d = table(name)["layernorm"][i]
-    report(f"layernorm {name} {d['rows']}x{d['cols']} split={d['split']} ns={ns}",
+    d = table(name, B)["layernorm"][i]
+    report(f"layernorm {name} b{B} {d['rows']}x{d['cols']} split={d['split']} ns={ns}",
            [layernorm_case(ops, d, 700 + i, ns)])
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("gate_split"))
-def test_gate(ops, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("gate_split"))
+def test_gate(ops, name, B, i, ns):
     """The gating stage of gated_conv1x1 at each decoder level: all T tasks in one launch, x = the level map (group
     P, offset 0), prompt logits [B, heads, T, T + P], channel logits of the 2C up-projection."""
-    d = table(name)["gate_split"][i]
-    report(f"gate {name} level C={d['C']} {d['gh']}x{d['gw']} ns={ns}", gate_case(ops, d, ns, name, seed=800 + i))
+    d = table(name, B)["gate_split"][i]
+    report(f"gate {name} b{B} level C={d['C']} {d['gh']}x{d['gw']} ns={ns}", gate_case(ops, d, ns, f"{name} b{B}", seed=800 + i))
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("bilinear", split=lambda d: d["form"] == "split"))
-def test_bilinear(ops, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("bilinear", split=lambda d: d["form"] == "split"))
+def test_bilinear(ops, name, B, i, ns):
     """The input downsample 1024x2048 -> 768x1536 (fp32 scale 4/3, inexact: ref_bilinear_any), the level x2
     up-samplings into split planes (f = 450, ld 456), the level sums into the 192 x 384 accumulator, the head resize
     384x768 -> 512x1024 (scale 0.75, exact)."""
-    d = table(name)["bilinear"][i]
-    report(f"bilinear {name} {d['h']}x{d['w']}->{d['H2']}x{d['W2']} {d['form']} ns={ns}",
+    d = table(name, B)["bilinear"][i]
+    report(f"bilinear {name} b{B} {d['h']}x{d['w']}->{d['H2']}x{d['W2']} {d['form']} ns={ns}",
            [bilinear_case(ops, d, ns, 900 + i)])
     torch.cuda.empty_cache()
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("bilinear_postproc", split=False))
-def test_bilinear_postproc(ops, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("bilinear_postproc", split=False))
+def test_bilinear_postproc(ops, name, B, i, ns):
     """predict()'s final resize fused with get_output: semseg argmax over 19 classes exact where the float64 top-2
     margin exceeds twice the logit bound, depth (kind 4) within the logit bound."""
-    d = table(name)["bilinear_postproc"][i]
+    d = table(name, B)["bilinear_postproc"][i]
     r = postproc_case(ops, d, 950 + i)
     if r is not None:
-        report(f"bilinear_postproc {name} kind {d['kind']}", [r])
+        report(f"bilinear_postproc {name} b{B} kind {d['kind']}", [r])
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,i,ns", entries("nhwc_to_nchw", split=False))
-def test_nhwc_to_nchw(ops, name, i, ns):
+@pytest.mark.parametrize("name,B,i,ns", entries("nhwc_to_nchw", split=False))
+def test_nhwc_to_nchw(ops, name, B, i, ns):
     """The 3ddet level maps and the backbone features (f = 450 of ld 456) to NCHW: bit-exact."""
-    d = table(name)["nhwc_to_nchw"][i]
+    d = table(name, B)["nhwc_to_nchw"][i]
     x = torch.full((d["B"] * d["H"] * d["W"], d["ld_in"]), float("nan"), device="cuda")
     x[:, :d["Cd"]] = randn(gen(980 + i), d["B"] * d["H"] * d["W"], d["Cd"])
     gb = Guarded((d["B"], d["Cd"], d["H"], d["W"]), torch.float32)

@@ -64,7 +64,7 @@ def test_swin_state_dict_matches_reference_names():
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["tps_tiny", "tps_tiny4"])
 def test_swin_golden_parity(cuda_dev, name):
-    from test_taskprompter_gpu import _check
+    from model_checks import check_parity as _check
 
     fx = torch.load(os.path.join(GOLD, f"{name}.pt"), weights_only=False)
     cfg, sd, m = _model(fx["cfg"], fx["seed"])
@@ -77,7 +77,7 @@ def test_swin_golden_parity(cuda_dev, name):
 
 @pytest.mark.gpu
 def test_swin_reference_window_geometry_and_graph_replay(cuda_dev):
-    from test_taskprompter_gpu import _check
+    from model_checks import check_parity as _check
 
     cfg, sd, m = _model("tps_mid", 13, graph=True)
     m = m.cuda()

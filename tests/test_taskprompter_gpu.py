@@ -12,6 +12,7 @@ import os
 import pytest
 import torch
 
+from model_checks import check_parity as _check
 from oracle import configs
 from oracle import taskprompter_ref as TPR
 
@@ -26,24 +27,6 @@ def _build(cfg, sd, nsplit, graph):
     m = TP.build_from_config(cfg, nsplit=nsplit, use_graph=graph).eval()
     m.load_state_dict(sd, strict=True)
     return m.cuda()
-
-
-def _check(got, ref, tasks, rel_l2, max_rel, check_argmax=True):
-    for t in tasks:
-        g, r = got[t].float().cpu(), ref[t].float()
-        assert g.shape == r.shape
-        assert torch.isfinite(g).all(), t
-        e2 = ((g - r).norm() / r.norm()).item()
-        em = ((g - r).abs().max() / r.abs().max()).item()
-        assert e2 < rel_l2, f"{t}: rel-L2 {e2:.3e}"
-        assert em < max_rel, f"{t}: max-abs/max {em:.3e}"
-        if check_argmax and r.shape[1] > 1:
-            top2 = r.topk(2, dim=1).values
-            margin = top2[:, 0] - top2[:, 1]
-            safe = margin > 1e-4 * r.abs().max()
-            agree = g.argmax(1) == r.argmax(1)
-            assert agree[safe].all(), f"{t}: argmax differs at {(~agree & safe).sum().item()} safe pixels"
-            assert agree.float().mean().item() > 0.999, f"{t}: argmax agreement {agree.float().mean().item():.5f}"
 
 
 @pytest.mark.parametrize("name", ["tp_tiny", "tp_tiny1", "tp_tiny_de"])

@@ -1,10 +1,14 @@
 """The wgmma GEMM, the implicit-GEMM convolution and the fused attention at every geometry the benched plans launch,
 against float64, element by element.
 
-Recording. A module fixture builds each benched plan (tp_cfg4, tp_cfg2, tp_cfg5, ip_cfg3, tps_swinB at
-bench.DEFAULT_BATCH, nsplit = 2, no graph) and the three-task tps_swinB3d (batch 1, nn.Identity as the 3ddet head: its
-window GEMMs have M = nW (3 + 144) rows) and runs one eager forward; tp_cfg4 and tp_cfg2 also run one eager
-TrainStep._fwd_bwd with the bench's criterion and labels. Pass-through recorders around ops.gemm, gemm_grouped,
+Recording. A module fixture builds the plan of every forward / predict() run of plan_calls.RUNS (nsplit = 2, no
+graph) at the run's batch -- tp_cfg4, tp_cfg2, tp_cfg5, ip_cfg3, tps_swinB at bench.DEFAULT_BATCH, the three-task
+tps_swinB3d at batch 1 and 4 (nn.Identity as the 3ddet head: its window GEMMs have M = B nW (3 + 144) rows), the
+reference's own model configs tp_nyud_vitL, tp_pascal_vitB, ip_nyud_vitL and tp_cfg4 / ip_cfg3 at its validation batch
+6, the PASCAL ones at the ragged last validation batch 5 -- and runs one eager forward; every training run (tp_cfg4 and
+tp_cfg2 at batch 4; tp_cfg4, tp_pascal_vitB, tp_nyud_vitL at the reference's training batch 2) runs one eager
+TrainStep._fwd_bwd with the bench's criterion and labels. The batch sets every GEMM's M, so its tile count and
+stream-K split. Pass-through recorders around ops.gemm, gemm_grouped,
 gemm_splitk, attention and the five composites of csrc/block_ops.cu turn every call into a geometry key (call_key): the
 shapes, the mode, the epilogue (act, bias, residual kind), the row maps (regroup, a_gather), the offsets, which outputs
 are written and every leading dimension. The same runs are bracketed by ops.profile_begin / profile_end, and every
@@ -94,7 +98,7 @@ import torch.nn.functional as F
 import kernel_cases as X
 from f64_checks import (SENTINEL, SPLIT, SPLIT_ABS, U, bits, check, mtt_ops, planes, sentinel, sentinel_split,
                         split_bound, sum_tol)
-from plan_calls import frozen, recording
+from plan_calls import frozen, recording, run_id, runs
 
 pytestmark = [pytest.mark.timeout(1500)]   # the GPU tests are marked one by one: the CPU self-checks are not
 
@@ -104,9 +108,8 @@ EX2 = 2.0 ** -21          # relative error of ex2.approx.ftz.f32
 F64_REF = 2.0 ** -53      # float64 unit roundoff: the reference's own rounding (see the docstring)
 TEETH_FRAC = 0.10
 TAIL_STAGES = 32          # keys with at most this many K-stages must show the ragged-tail defect (see the docstring)
-FORWARD = ["tp_cfg4", "tp_cfg2", "tp_cfg5", "ip_cfg3", "tps_swinB", "tps_swinB3d"]
-EXTRA_BATCH = {"tps_swinB3d": 1}   # forwards the bench does not run: their batch
-TRAIN = ["tp_cfg4", "tp_cfg2"]
+FORWARD = runs(("forward", "predict"))     # (config, batch): one recorded forward each
+TRAIN = runs(("train",))
 RECORDED = ["gemm", "gemm_grouped", "gemm_splitk", "attention", "ln_qkv", "proj_residual", "ln_mlp_residual",
             "gated_conv1x1", "conv3x3_bn_act"]
 
@@ -928,26 +931,24 @@ def _record_run(ops, fn):
     return seen, [tuple(int(v) for v in r[:4]) for r in prof]
 
 
-def _forward(name, dev, nsplit):
-    import bench
+def _forward(name, B, dev, nsplit):
     ops = mtt_ops()
     cfg, model = _build(name, dev, nsplit)
     model.eval()
-    x = torch.randn(EXTRA_BATCH.get(name) or bench.DEFAULT_BATCH[name], 3, *cfg["img_size"], device=dev)
+    x = torch.randn(B, 3, *cfg["img_size"], device=dev)
     out = _record_run(ops, lambda: model(x))
     del model
     torch.cuda.empty_cache()
     return out
 
 
-def _train(name, dev):
+def _train(name, B, dev):
     import bench
     from mtt_b200.train import TrainStep
     ops = mtt_ops()
     cfg, model = _build(name, dev, 2)
     ts = TrainStep(model, nsplit=2, use_graph=False)
     crit, _ = bench._train_criterion(cfg)
-    B = bench.DEFAULT_BATCH[name]
     g = torch.Generator().manual_seed(1)
     x = torch.randn(B, 3, *cfg["img_size"], generator=g).to(dev)
     y = {t: v.to(dev) for t, v in bench._train_labels(cfg, B, g).items()}
@@ -959,15 +960,15 @@ def _train(name, dev):
 
 @pytest.fixture(scope="module")
 def recorded(cuda_dev):
-    """{(config, "forward" | "train" | "forward_speed"): (recorded keys in call order, profiled launches)}."""
+    """{(config, batch, "forward" | "train" | "forward_speed"): (recorded keys in call order, profiled launches)}."""
     mtt_ops()
-    runs = {}
-    for name in FORWARD:
-        runs[(name, "forward")] = _forward(name, cuda_dev, 2)
-    runs[("tp_cfg4", "forward_speed")] = _forward("tp_cfg4", cuda_dev, 1)
-    for name in TRAIN:
-        runs[(name, "train")] = _train(name, cuda_dev)
-    return runs
+    out = {}
+    for name, B in FORWARD:
+        out[(name, B, "forward")] = _forward(name, B, cuda_dev, 2)
+    out[("tp_cfg4", 4, "forward_speed")] = _forward("tp_cfg4", 4, cuda_dev, 1)
+    for name, B in TRAIN:
+        out[(name, B, "train")] = _train(name, B, cuda_dev)
+    return out
 
 
 def distinct(seq):
@@ -979,32 +980,60 @@ def distinct(seq):
 def test_recording_explains_every_launch(recorded):
     """Every profiled tensor-core launch of every recorded run is issued by a recorded call, and every recorded call
     issued the launches it should: the multisets are equal."""
-    for (name, part), (seen, prof) in recorded.items():
-        assert seen, f"{name} {part}: nothing recorded"
+    for (name, B, part), (seen, prof) in recorded.items():
+        assert seen, f"{name} b{B} {part}: nothing recorded"
         want = collections.Counter(l for k in seen for l in launches_of(k))
         got = collections.Counter(prof)
         extra, missing = got - want, want - got
-        assert not extra, f"{name} {part}: launches no recorded call explains: {sorted(extra.items())[:6]}"
-        assert not missing, f"{name} {part}: recorded calls whose launches were not profiled: {sorted(missing.items())[:6]}"
-        print(f"{name} {part}: {len(seen)} calls, {len(distinct(seen))} distinct keys, {len(prof)} tensor-core launches")
+        assert not extra, f"{name} b{B} {part}: launches no recorded call explains: {sorted(extra.items())[:6]}"
+        assert not missing, (f"{name} b{B} {part}: recorded calls whose launches were not profiled: "
+                             f"{sorted(missing.items())[:6]}")
+        print(f"{name} b{B} {part}: {len(seen)} calls, {len(distinct(seen))} distinct keys, {len(prof)} tensor-core "
+              f"launches")
+    assert {(n, B, "forward") for n, B in FORWARD} | {(n, B, "train") for n, B in TRAIN} <= set(recorded)
+    _assert_reaches(recorded)
+
+
+def _fields(key):
+    """The field dicts of a key (one per problem of a grouped GEMM)."""
+    return [dict(p) for p in key[1]] if key[0] == "gemm" else [dict(key[1])]
+
+
+def _assert_reaches(recorded):
+    """The runs reach the geometries they are in the list for."""
+    keys = lambda name, B, part="forward": distinct(recorded[(name, B, part)][0])
+    # ip_nyud_vitL: 7 x 9 key maps, Tk = 4 * 63 = 252 at every stage: the grouped QK^T has N = 252 and the grouped
+    # P.V has K = 252 (a 60-deep last K-stage; ip_cfg3's 320 = 5 x 64 has none)
+    ip = [f for k in keys("ip_nyud_vitL", 6) if k[0] == "gemm" and len(k[1]) > 1 for f in _fields(k)]
+    assert any(f["K"] == 252 for f in ip) and any(f["N"] == 252 for f in ip), "ip_nyud_vitL: no Tk = 252 GEMM"
+    # tp_nyud_vitL: attention over N = 4 + 28 * 36 = 1012 tokens at 16 heads, 6 images
+    att = [dict(k[1]) for k in keys("tp_nyud_vitL", 6) if k[0] == "attention"]
+    assert {(f["B"], f["N"], f["H"]) for f in att} == {(6, 1012, 16)}, att
+    # tp_pascal_vitB: e = 780 columns per gate, the channel gate's at column 784, and f = 1024; tp_cfg4 at valBatch 6:
+    # M = 6 * 1029
+    gc = [dict(k[1]) for k in keys("tp_pascal_vitB", 6) if k[0] == "gated_conv1x1"]
+    assert gc and {(f["e"], f["chan_col"]) for f in gc} == {(780, 784)}, gc
+    assert any(f["N"] == 1024 for k in keys("tp_pascal_vitB", 6) if k[0] == "gemm" for f in _fields(k))
+    assert any(dict(k[1])["x"][0] == 6 * 1029 for k in keys("tp_cfg4", 6) if k[0] == "ln_qkv")
+    assert any(f["M"] == 2 * 1029 for k in keys("tp_pascal_vitB", 2, "train") if k[0] == "gemm" for f in _fields(k))
 
 
 @pytest.mark.gpu
 def test_speed_mode_plan_records_the_same_keys(recorded):
     """tp_cfg4 built with nsplit = 1 issues the same geometries apart from the plane counts: a speed-mode replay of
     the parity keys covers the speed-mode plan."""
-    par = {without_planes(k) for k in recorded[("tp_cfg4", "forward")][0]}
-    spd = {without_planes(k) for k in recorded[("tp_cfg4", "forward_speed")][0]}
+    par = {without_planes(k) for k in recorded[("tp_cfg4", 4, "forward")][0]}
+    spd = {without_planes(k) for k in recorded[("tp_cfg4", 4, "forward_speed")][0]}
     assert par == spd, (sorted(par - spd, key=str)[:3], sorted(spd - par, key=str)[:3])
-    modes = {dict(k[1] if k[0] != "gemm" else k[1][0])["nsplit"] for k in recorded[("tp_cfg4", "forward_speed")][0]}
+    modes = {dict(k[1] if k[0] != "gemm" else k[1][0])["nsplit"] for k in recorded[("tp_cfg4", 4, "forward_speed")][0]}
     assert modes == {1}, modes
 
 
-def _replay_all(recorded, name, part, dev):
+def _replay_all(recorded, name, B, part, dev):
     ops = mtt_ops()
     ops.set_gemm_variant(0)
     ops.set_gemm_streamk(1)
-    keys = distinct(recorded[(name, part)][0])
+    keys = distinct(recorded[(name, B, part)][0])
     worst = collections.defaultdict(float)
     speed, tail, attn = [], [], []
     t0 = time.time()
@@ -1025,7 +1054,7 @@ def _replay_all(recorded, name, part, dev):
             speed += [t[0] for t in th if t[0] is not None]
             tail += [t[1:] for t in th]
         torch.cuda.empty_cache()
-    print(f"\n{name} {part}: {len(keys)} distinct keys replayed in {time.time() - t0:.0f} s")
+    print(f"\n{name} b{B} {part}: {len(keys)} distinct keys replayed in {time.time() - t0:.0f} s")
     for k in sorted(worst):
         print(f"  worst err/bound {k:16s} {worst[k]:.3f}")
     fractions = (("speed-mode teeth", speed),
@@ -1037,15 +1066,15 @@ def _replay_all(recorded, name, part, dev):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", FORWARD)
-def test_forward_launches_f64(recorded, cuda_dev, name):
-    _replay_all(recorded, name, "forward", cuda_dev)
+@pytest.mark.parametrize("name,B", [pytest.param(n, B, id=run_id(n, B)) for n, B in FORWARD])
+def test_forward_launches_f64(recorded, cuda_dev, name, B):
+    _replay_all(recorded, name, B, "forward", cuda_dev)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", TRAIN)
-def test_train_launches_f64(recorded, cuda_dev, name):
-    _replay_all(recorded, name, "train", cuda_dev)
+@pytest.mark.parametrize("name,B", [pytest.param(n, B, id=run_id(n, B)) for n, B in TRAIN])
+def test_train_launches_f64(recorded, cuda_dev, name, B):
+    _replay_all(recorded, name, B, "train", cuda_dev)
 
 
 # ---- CPU self-checks ---------------------------------------------------------------------------------------------------------

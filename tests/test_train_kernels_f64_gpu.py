@@ -1,8 +1,10 @@
 """-m gpu: the training-step kernels (csrc/train_ops.cu) and the loss kernels (csrc/losses.cu) at the geometries the
-training step of tp_cfg4 (ViT-L, PASCAL, 5 tasks) and tp_cfg2 (ViT-B, NYUD, 4 tasks) really runs, against float64
-references written from each operation's definition: torch autograd in float64 for the adjoints, F.batch_norm /
-clip_grad_norm_ / torch.optim.Adam in float64, oracle/loss_ref.py in float64. Then the whole tp_cfg2_d4 reverse pass
-against autograd of the train-mode restatement.
+training runs of plan_calls.RUNS really run -- tp_cfg4 (ViT-L, PASCAL, 5 tasks) and tp_cfg2 (ViT-B, NYUD, 4 tasks) at
+batch 4, and at the reference's training batch 2 tp_cfg4 and its own tp_pascal_vitB (ViT-B, 4 x 4 channel windows with
+ctr, f = 1024) and tp_nyud_vitL (ViT-L, 4 x 4 channel windows, f = 768) -- against float64 references written from
+each operation's definition: torch autograd in float64 for the adjoints, F.batch_norm / clip_grad_norm_ /
+torch.optim.Adam in float64, oracle/loss_ref.py in float64. Then the whole tp_cfg2_d4 reverse pass against autograd of
+the train-mode restatement.
 
 Error model: tests/f64_checks.py. The BatchNorm statistics accumulate in double (U64 in place of u). Every assert below
 states which bound it uses."""
@@ -14,11 +16,13 @@ import torch.nn.functional as F
 
 from f64_checks import LAM, SPLIT, SPLIT_ABS, U, U64, check, gen, ops, randn, split_planes, sum_tol  # noqa: F401
 from oracle import configs, loss_ref
-from plan_calls import TPGeom
+from model_checks import reverse_pass_errors
+from plan_calls import TPGeom, run_id, runs
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 
-CONFIGS = ["tp_cfg4", "tp_cfg2"]
+TRAIN = runs(("train",))                                   # (config, batch)
+CONFIGS = list(dict.fromkeys(name for name, _ in TRAIN))   # the loss tests run each config's tasks at batch 2
 
 
 def _sms():
@@ -33,10 +37,10 @@ def colreduce_depth(rows, cols):
     return math.ceil(rows / (8 * rb)) + 8 + rb
 
 
-@pytest.fixture(scope="module", params=CONFIGS)
+@pytest.fixture(scope="module", params=[pytest.param(run, id=run_id(*run)) for run in TRAIN])
 def geom(request, cuda_dev):
     import mtt_b200  # noqa: F401
-    return TPGeom(request.param)
+    return TPGeom(*request.param)
 
 
 def split_of(ops, x):
@@ -612,9 +616,6 @@ def _loss_bounds(task, pred, label, gscale):
     return e_val + 1e-300, e_grad
 
 
-SIZES = {"tp_cfg4": (512, 512), "tp_cfg2": (448, 576)}
-
-
 @pytest.mark.parametrize("name", CONFIGS)
 def test_losses_at_the_training_sizes_f64(cuda_dev, name):
     """Every task loss of the config at its image size, batch 2, image 0 fully ignored: value and elementwise d loss / d
@@ -623,7 +624,7 @@ def test_losses_at_the_training_sizes_f64(cuda_dev, name):
     import mtt_b200  # noqa: F401
 
     cfg = configs.taskprompter(name)
-    H, W = SIZES[name]
+    H, W = cfg["img_size"]
     g = torch.Generator(device="cuda").manual_seed(20)
     for task in cfg["tasks"]:
         nout = cfg["num_output"][task]
@@ -736,53 +737,9 @@ def test_training_step_reverse_pass_tp_cfg2_d4(cuda_dev):
     """tp_cfg2_d4 (ViT-B width, 448 x 576, the 4 NYUD tasks, 4 x 4 channel windows, e = f = 768, no ctr), batch 2: the
     same d loss / d prediction through TrainStep.backward and through float64 autograd of the train-mode restatement
     (pinned to the reference by test_train.py::test_train_mode_restatement_is_pinned_to_the_reference), every parameter
-    gradient elementwise. DropPath draws come from a CPU generator in the reference's call order."""
-    import mtt_b200  # noqa: F401
-    from mtt_b200 import losses
-    from mtt_b200 import taskprompter as TP
-    from mtt_b200.train import TrainStep
-    from oracle import taskprompter_ref as TPR
-    from oracle.make_golden import train_inputs
-
-    cfg = configs.taskprompter("tp_cfg2_d4")
-    seed, B = 31, 2
-    sd = TPR.init_state_dict(cfg, seed=seed)
-    model = TP.build_from_config(cfg, use_graph=False)
-    model.load_state_dict(sd, strict=True)
-    model.to(cuda_dev)
-    ts = TrainStep(model)
-    n_act = sum(1 for r in torch.linspace(0, 0.15, cfg["depth"]) if float(r) > 0)
-    gcpu = torch.Generator().manual_seed(seed + 900)
-    masks = [torch.rand(B, 1, 1, generator=gcpu) for _ in range(4 * n_act)]
-    x, labels = train_inputs(cfg, seed, B)
-    ts.zero_grad()
-    with torch.no_grad():
-        out = ts.forward(x.to(cuda_dev), drop_rand=masks)
-    p = dict(TASKS=dict(NAMES=list(cfg["tasks"])), edge_w=0.95, ignore_index=255, ignore_invalid_area_depth=True,
-             loss_kwargs=dict(loss_weights={t: 1.0 for t in cfg["tasks"]}))
-    leaves = {t: out[t].detach().requires_grad_(True) for t in cfg["tasks"]}
-    loss = losses.get_criterion(p)(leaves, {t: v.to(cuda_dev) for t, v in labels.items()}, tasks=cfg["tasks"])
-    grads = dict(zip(cfg["tasks"], torch.autograd.grad(loss["total"], [leaves[t] for t in cfg["tasks"]])))
-    with torch.no_grad():
-        ts.backward(grads)
-    torch.cuda.synchronize()
-    # float64 autograd of the train-mode restatement with the same draws and the same d loss / d prediction
-    sdd = {k: (v.to(cuda_dev).double() if v.is_floating_point() else v.to(cuda_dev)) for k, v in sd.items()}
-    params = {k: v.requires_grad_(True) for k, v in sdd.items() if v.is_floating_point() and "running_" not in k}
-    with TPR.train_mode(0.15, rand=[m.to(cuda_dev).double() for m in masks]):
-        ref_out = TPR.forward(sdd, cfg, x.to(cuda_dev).double())
-    for t in cfg["tasks"]:
-        err = ((out[t].double() - ref_out[t].detach()).norm() / ref_out[t].detach().norm()).item()
+    gradient elementwise (tests/model_checks.py reverse_pass_errors). DropPath draws come from a CPU generator in the
+    reference's call order."""
+    fwd, bad, n = reverse_pass_errors("tp_cfg2_d4", cuda_dev, seed=31, B=2)
+    for t, err in fwd.items():
         assert err < 2e-4, f"train-mode forward {t}: rel-L2 {err:.3e}"
-    torch.autograd.backward([ref_out[t] for t in cfg["tasks"]], [grads[t].double() for t in cfg["tasks"]])
-    og = {k: (v.grad if v.grad is not None else torch.zeros_like(v)) for k, v in params.items()}
-    total = math.sqrt(sum(float((g ** 2).sum()) for g in og.values()))
-    floor = 1e-4 * total
-    bad = []
-    for k, ref in og.items():
-        # split-bf16 GEMMs (2^-17 relative per operand) chained through 4 blocks and the decoder: the same 2e-3 rel-L2
-        # as the tp_cfg4_d4 reverse pass, with the floor for parameters whose gradient is zero up to noise
-        err = (ts.G_(k).double() - ref).norm().item() / max(ref.norm().item(), floor)
-        if not err < 2e-3:
-            bad.append((k, err))
-    assert not bad, f"{len(bad)} of {len(og)} parameter gradients off: {sorted(bad, key=lambda kv: -kv[1])[:8]}"
+    assert not bad, f"{len(bad)} of {n} parameter gradients off: {bad[:8]}"
