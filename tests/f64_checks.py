@@ -64,6 +64,18 @@ def report(name, ratios):
     print(f"{name}: worst error / bound = {max(ratios):.3f}")
 
 
+def bce_rel(x):
+    """Relative bound of the fp32 softplus / sigmoid of logit x in the balanced BCE (loss_terms.cuh balanced_bce_term):
+    (|x| + 8) u. x is a float64 tensor."""
+    return (x.abs() + 8) * U
+
+
+def bce_term_bound(x):
+    """Bound of one fp32 balanced BCE term at logit x (label in [0, 1], weight in [0, 1)): bce_rel(x) of a term no larger
+    than |x| + 1."""
+    return bce_rel(x) * (x.abs() + 1)
+
+
 # ---- split planes --------------------------------------------------------------------------------------------------------
 def split_planes(x, ns=2):
     """The planes the kernels write for fp32 x: hi = bf16(x) (round to nearest even), lo = bf16(x - hi)."""

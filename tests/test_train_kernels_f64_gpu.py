@@ -14,7 +14,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from f64_checks import LAM, SPLIT, SPLIT_ABS, U, U64, check, gen, ops, randn, split_planes, sum_tol  # noqa: F401
+from f64_checks import (LAM, SPLIT, SPLIT_ABS, U, U64, bce_rel, bce_term_bound, check, gen, ops, randn,  # noqa: F401
+                        split_planes, sum_tol)
 from oracle import configs, loss_ref
 from model_checks import reverse_pass_errors
 from plan_calls import TPGeom, run_id, runs
@@ -600,9 +601,8 @@ def _loss_bounds(task, pred, label, gscale):
     elif task == "edge":
         keep = (y != ign)
         nv = max(int(keep.sum()), 1)
-        k = (x.abs() + 8) * U
-        e_grad = k * gscale * keep / nv
-        e_val = float((k * (x.abs() + 1) * keep).sum()) / nv
+        e_grad = bce_rel(x) * gscale * keep / nv
+        e_val = float((bce_term_bound(x) * keep).sum()) / nv
     else:
         keep = (y != ign).all(1, keepdim=True)
         nv = max(int(keep.sum()), 1)
