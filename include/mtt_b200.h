@@ -616,7 +616,11 @@ int mtt_nms_bev(const float* boxes, int32_t n, float thresh, int32_t rotated, in
  * mtt_swin_merge_gather: [B,H,W,C] -> [B*(H/2)*(W/2), 4C], quadrant order (0,0), (1,0), (0,1), (1,1) (TP:441-447).
  * mtt_conv3x3_s2_maps: stride-2 3x3 conv (pad 1) over maps stored as in[b, ci, in_offset + y*W + x] with channel stride
  *   in_stride (PatchMerging.spa_attn_ds on the logit maps, TP:458-460). w [Cout, Cin, 3, 3].
- * mtt_swin_chan_up: out[bt, o, win] = sum_c w[o, c] raw_chan[bt, c, win] (process_chan_attn, TP:463-466). */
+ * mtt_swin_chan_up: out[bt, o, win] = sum_c w[o, c] raw_chan[bt, c, win] (process_chan_attn, TP:463-466).
+ * mtt_swin_logit_maps: the prompt-row logit maps between the gating layout logits [rows, T + L] (map r at columns
+ *   [T, T + L)) and the reference's raw_spa_attn [B, heads, T, H, W] = maps [rows, L], rows = B*heads*T <= 65535.
+ *   to_maps != 0: src = logits, dst = maps; to_maps = 0: src = maps, dst = logits (its columns < T are not written).
+ *   The sub-module forwards' layout change (SwinTransformerBlock / PatchMerging, TP:352-365, :453-460). */
 int mtt_swin_window_gather(const float* xn, int64_t ldx, const float* pn, int64_t ldp, int32_t B, int32_t H, int32_t W,
                            int32_t C, int32_t T, int32_t ws, int32_t shift, void* out_hi, void* out_lo, int64_t ld_out,
                            mtt_stream_t stream);
@@ -640,6 +644,8 @@ int mtt_conv3x3_s2_maps(const float* in, const float* w, const float* bias, int3
                         mtt_stream_t stream);
 int mtt_swin_chan_up(const float* raw_chan, const float* w, int32_t BT, int32_t C, int32_t Cout, int32_t nwin, float* out,
                      mtt_stream_t stream);
+int mtt_swin_logit_maps(const float* src, float* dst, int32_t rows, int32_t T, int32_t L, int32_t to_maps,
+                        mtt_stream_t stream);
 
 /* ---- layout changes at the nn.Module boundaries (ConvHead.forward takes / returns NCHW like the reference) ---- */
 int mtt_nchw_to_nhwc_split(const float* in, int32_t B, int32_t C, int32_t H, int32_t W, void* out_hi, void* out_lo,

@@ -371,6 +371,20 @@ chan_up_kernel(const float* __restrict__ rc, const float* __restrict__ w, int BT
   }
 }
 
+// ---- prompt-row logit maps between the gating layout and the reference's raw_spa_attn ----------------------------------
+// logits [rows, T + L] holds map r at columns [T, T + L); maps [rows, L] is the reference's [B, heads, T, H, W]. One block
+// row per map, consecutive threads on consecutive columns of both sides: coalesced reads and writes. to_maps = 0 writes
+// the logits' map columns only (their first T columns are not part of the map and stay as they are).
+__global__ void __launch_bounds__(256)
+swin_logit_maps_kernel(const float* __restrict__ src, float* __restrict__ dst, int T, int L, int to_maps) {
+  const long long r = blockIdx.y;
+  const long long ld_src = to_maps ? T + L : L, ld_dst = to_maps ? L : T + L;
+  const int off_src = to_maps ? T : 0, off_dst = to_maps ? 0 : T;
+  const float* s = src + r * ld_src + off_src;
+  float* d = dst + r * ld_dst + off_dst;
+  for (int l = blockIdx.x * blockDim.x + threadIdx.x; l < L; l += gridDim.x * blockDim.x) d[l] = s[l];
+}
+
 static int make_geom(WinGeom& g, int B, int H, int W, int C, int T, int ws, int shift) {
   if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || T < 0 || ws <= 0 || shift < 0 || shift >= ws)
     return set_error(MTT_ERR_BAD_SHAPE, "swin: bad window geometry (B=%d %dx%d C=%d T=%d ws=%d shift=%d)", B, H, W, C, T, ws,
@@ -530,6 +544,15 @@ int mtt_swin_chan_up(const float* raw_chan, const float* w, int32_t BT, int32_t 
   const long long n = (long long)BT * Cout * nwin;
   chan_up_kernel<<<(unsigned)((n + 255) / 256), 256, 0, STREAM>>>(raw_chan, w, BT, C, Cout, nwin, out);
   return check_launch("mtt_swin_chan_up");
+}
+
+int mtt_swin_logit_maps(const float* src, float* dst, int32_t rows, int32_t T, int32_t L, int32_t to_maps,
+                        mtt_stream_t stream) {
+  if (!src || !dst || rows <= 0 || rows > 65535 || T < 0 || L <= 0)
+    return set_error(MTT_ERR_BAD_SHAPE, "mtt_swin_logit_maps: bad arguments (rows=%d T=%d L=%d)", rows, T, L);
+  const int bx = (L + 255) / 256 < 64 ? (L + 255) / 256 : 64;
+  swin_logit_maps_kernel<<<dim3(bx, rows), 256, 0, STREAM>>>(src, dst, T, L, to_maps ? 1 : 0);
+  return check_launch("mtt_swin_logit_maps");
 }
 
 }  // extern "C"

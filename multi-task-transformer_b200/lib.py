@@ -202,6 +202,7 @@ SYMBOLS = {
     "mtt_swin_merge_gather": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _i64, _vp]),
     "mtt_conv3x3_s2_maps": (C.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i64, _i32, _i64, _i32, _vp, _vp]),
     "mtt_swin_chan_up": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp]),
+    "mtt_swin_logit_maps": (C.c_int, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
     "mtt_nchw_to_nhwc_split": (C.c_int, [_vp, _i32, _i32, _i32, _i32, _vp, _vp, _i64, _vp]),
     "mtt_nhwc_to_nchw": (C.c_int, [_vp, _i64, _i32, _i32, _i32, _i32, _vp, _vp]),
     # training step (csrc/train_ops.cu)

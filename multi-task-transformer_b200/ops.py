@@ -772,6 +772,18 @@ def swin_chan_up(rc_in, w, out, *, BT, Cdim, nwin):
     _launch("mtt_swin_chan_up", _ptr(rc_in), _ptr(w), BT, Cdim, w.shape[0], nwin, _ptr(out))
 
 
+def swin_logit_maps(logits, maps, *, T, to_maps):
+    """Prompt-row logit maps between the gating layout logits [B, heads, T, T + H*W] (the map at column T on) and the
+    reference's raw_spa_attn maps [B, heads, T, H, W]; to_maps: logits -> maps, else maps -> logits (the first T
+    columns of the logits are not written)."""
+    assert logits.is_contiguous() and maps.is_contiguous() and logits.dtype == maps.dtype == torch.float32
+    L = logits.shape[-1] - T
+    rows = logits.numel() // logits.shape[-1]
+    assert maps.numel() == rows * L
+    src, dst = (logits, maps) if to_maps else (maps, logits)
+    _launch("mtt_swin_logit_maps", _ptr(src), _ptr(dst), rows, T, L, 1 if to_maps else 0)
+
+
 # ---- training step (csrc/train_ops.cu): fp32 [rows, cols] tensors, last dim contiguous ----------------------------------
 def _ld(t):
     assert t.dtype == torch.float32 and t.stride(-1) == 1

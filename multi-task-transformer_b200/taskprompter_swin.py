@@ -35,6 +35,10 @@ fea_fuse at each level. Its level features stay at the level's own resolution (n
 fused across scales (no multi_scale_fuse['3ddet'], TP:635, :709-710): the plan writes them as 4 NCHW maps
 [B, f, h_l, w_l], and TaskPrompterWrapper hands them to heads['3ddet'] -- the reference's FCOS3DHead (mmcv / mmdet3d), or any
 module -- which runs in PyTorch on the same stream. The library has no kernels for that head.
+SwinTransformerBlock, PatchMerging and BasicLayer also have the reference's forwards (TP:310-405, :430-477, :527-537),
+tensors in and out in its layouts: they run the plan's block and merge launch code (_launch_swin_block, _launch_merge)
+eagerly on a _StageSpace sized for the call, with the same packed weights. WindowAttention.forward raises: the reference
+returns the full pre-softmax window map from it, which the fused kernel never forms (SURVEY.md section 8b).
 Unsupported (raises): absolute position embedding (ape=True; no reference config uses it). Eval mode only.
 """
 import math
@@ -44,7 +48,8 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .plans import Plan, _cached, _check_input, _dev_ctx, _f32, _lin, _pack_stem, _plan_for, _predict_outputs
+from .plans import (Plan, _cached, _check_input, _dev_ctx, _f32, _lin, _pack_stem, _plan_for, _predict_outputs,
+                    _Streams)
 from .taskprompter import (PARITY, Mlp, PatchEmbed, _HeadSpace, _launch_head, _mirror_head, _pack_fuse, _pack_head,
                            _trunc_normal_)
 
@@ -89,6 +94,12 @@ class WindowAttention(nn.Module):
         self.proj = nn.Linear(dim, dim)
         _trunc_normal_(self.relative_position_bias_table, std=.02)
 
+    def forward(self, *args, **kwargs):
+        raise NotImplementedError(
+            "mtt_b200 WindowAttention has no forward: the reference's returns the full (B*nW, heads, T + ws^2, T + ws^2) "
+            "pre-softmax map, which the fused window-attention kernel never forms (it keeps only the prompt rows, "
+            "SURVEY.md H4). Call SwinTransformerBlock.forward: its raw_spa_attn holds those rows on the map")
+
 
 class SwinTransformerBlock(nn.Module):
     def __init__(self, last_block, p, dim, input_resolution, num_heads, window_size=7, shift_size=0, mlp_ratio=4.,
@@ -116,6 +127,25 @@ class SwinTransformerBlock(nn.Module):
         if not last_block:
             self.chan_proj = nn.Linear(ce, ce)
             self.token_trans1 = nn.Linear(ce, dim)
+        self.chan_nheads = p.chan_nheads
+
+    nsplit = PARITY
+
+    def forward(self, x, task_prompts):
+        """TP:310-405: (x [B, H*W, C], [raw_spa_attn [B, heads, T, H, W], raw_chan_attn [B, T, C, nh, nw]],
+        task_prompts [B, T, C]), fresh tensors. The model's last block (LAST_BLOCK_FLAG) does not update the prompts and
+        returns their window-averaged attention outputs, as the reference does (:344, :399-405)."""
+        _check_input(self, x)
+        B, T = _check_tokens(self, x, task_prompts, self.dim)
+        dev, ns = x.device, self.nsplit
+        with _dev_ctx(dev):
+            w = _pack_swin_block(self, dev, ns)
+            s = _module_space(self, self, B, T, dev, ns)
+            _load(s, x, task_prompts)
+            spa = torch.zeros(B, T, self.dim, device=dev) if self.LAST_BLOCK_FLAG else None
+            _launch_swin_block(s, w, self.shift_size, None if spa is None else spa.view(B * T, self.dim))
+            return (s.x.view(B, s.L, s.C).clone(), _attn_out(s, s.logits, s.rc, s.H, s.W),
+                    spa if spa is not None else s.p.view(B, T, s.C).clone())
 
 
 class PatchMerging(nn.Module):
@@ -128,6 +158,30 @@ class PatchMerging(nn.Module):
         self.process_chan_attn = nn.Linear(dim, 2 * dim, bias=False)
         self.task_prompts_up = nn.Linear(dim, 2 * dim, bias=False)
         self.spa_attn_ds = nn.Conv2d(num_heads * T, num_heads * T, kernel_size=3, padding=1, stride=2)
+        self.num_heads, self.chan_nheads = num_heads, p.chan_nheads
+
+    nsplit = PARITY
+
+    def forward(self, x, task_prompts, attn_weight):
+        """TP:430-477: (x [B, H/2*W/2, 2C], task_prompts [B, T, 2C], [raw_spa_attn [B, heads, T, H/2, W/2],
+        raw_chan_attn [B, T, 2C, nh, nw]]), fresh tensors, from attn_weight = [raw_spa_attn [B, heads, T, H, W],
+        raw_chan_attn [B, T, C, nh, nw]] of the stage's last block."""
+        _check_input(self, x)
+        B, T = _check_tokens(self, x, task_prompts, self.dim)
+        raw_spa, raw_chan = attn_weight
+        H, W = self.input_resolution
+        C, nh = self.dim, int(round(math.sqrt(self.chan_nheads)))
+        if tuple(raw_spa.shape) != (B, self.num_heads, T, H, W) or tuple(raw_chan.shape) != (B, T, C, nh, nh):
+            raise ValueError(f"PatchMerging: expected attn_weight [[{B},{self.num_heads},{T},{H},{W}], [{B},{T},{C},{nh},"
+                             f"{nh}]], got {[tuple(raw_spa.shape), tuple(raw_chan.shape)]}")
+        dev, ns = x.device, self.nsplit
+        with _dev_ctx(dev):
+            w = _pack_merge(self, dev, ns)
+            s = _module_space(self, None, B, T, dev, ns)
+            _load(s, x, task_prompts)
+            ops.swin_logit_maps(s.logits, raw_spa.to(device=dev, dtype=torch.float32).contiguous(), T=T, to_maps=False)
+            s.rc.copy_(raw_chan)
+            return _launch_merge_out(s, w)
 
 
 class BasicLayer(nn.Module):
@@ -138,6 +192,29 @@ class BasicLayer(nn.Module):
             SwinTransformerBlock(last_layer and i == depth - 1, p, dim, input_resolution, num_heads, window_size,
                                  0 if i % 2 == 0 else window_size // 2, mlp_ratio, qkv_bias) for i in range(depth)])
         self.downsample = PatchMerging(p, num_heads, input_resolution, dim) if downsample else None
+
+    nsplit = PARITY
+
+    def forward(self, x, task_prompts):
+        """TP:527-537: the blocks in turn, then the PatchMerging if there is one: (x, attn_weight, task_prompts) as the
+        last of them returns them (attn_weight = [raw_spa_attn, raw_chan_attn]), fresh tensors. The stage runs on one
+        workspace: its maps go from block to block and into the merge without leaving the plan's layout."""
+        _check_input(self, x)
+        blk0 = self.blocks[0]
+        B, T = _check_tokens(self, x, task_prompts, blk0.dim)
+        dev, ns = x.device, self.nsplit
+        with _dev_ctx(dev):
+            Wb = [_pack_swin_block(blk, dev, ns) for blk in self.blocks]
+            s = _module_space(self, blk0, B, T, dev, ns)
+            _load(s, x, task_prompts)
+            spa = torch.zeros(B, T, blk0.dim, device=dev) if self.blocks[-1].LAST_BLOCK_FLAG else None
+            for blk, w in zip(self.blocks, Wb):
+                _launch_swin_block(s, w, blk.shift_size, None if spa is None else spa.view(B * T, blk0.dim))
+            if self.downsample is None:
+                return (s.x.view(B, s.L, s.C).clone(), _attn_out(s, s.logits, s.rc, s.H, s.W),
+                        spa if spa is not None else s.p.view(B, T, s.C).clone())
+            x, task_prompts, attn_weight = _launch_merge_out(s, _pack_merge(self.downsample, dev, ns))
+            return x, attn_weight, task_prompts
 
 
 class SwinPatchEmbed(PatchEmbed):
@@ -288,6 +365,158 @@ def chan_kv_chunks(rows, ce, L):
     return max(1, min(32, 148 // tiles, L // 512))
 
 
+class _StageSpace:
+    """Activations of one Swin stage for one batch size: the token map x [B*L, C] and prompts p [B*T, C] its blocks update
+    in place, their intermediates, the prompt-row logit maps in the gating layout logits [B, heads, T, T + L] and the
+    channel logits rc [B, T, C, nh, nw] of the last block, and (merge) the PatchMerging scratch and its down-sampled
+    maps logits_ds / rc_up. Shared by the blocks of a stage; the buffers only the blocks use are there when blk (a block of
+    the stage: window, MLP and channel-attention sizes) is given."""
+
+    def __init__(self, C, res, heads, B, T, chan_nheads, device, ns, streams, blk=None, merge=False):
+        S = lambda r, c, **kw: ops.Split(r, c, device, ns, **kw)
+        z = lambda *s: torch.zeros(*s, device=device, dtype=torch.float32)
+        self.B, self.T, self.ns, self.streams = B, T, ns, streams
+        self.nh = self.nw = int(round(math.sqrt(chan_nheads)))
+        self.C, self.heads = C, heads
+        self.H, self.W = res
+        self.L = L = self.H * self.W
+        self.x = z(B * L, C)
+        self.p = z(B * T, C)
+        self.ps = S(B * T, C)
+        self.logits = z(B, heads, T, T + L)                 # prompt-row logits in the gating kernel's layout
+        self.rc = z(B, T, C, self.nh, self.nw)
+        if blk is not None:
+            self.ce = ce = blk.chan_q.in_features
+            self.ws = ws = blk.window_size
+            self.Hp, self.Wp = blk.padded
+            self.nW = nW = (self.Hp // ws) * (self.Wp // ws)
+            self.wl = wl = ws * ws
+            self.rows_w = rows_w = B * nW * (T + wl)
+            self.xn32, self.pn32 = z(B * L, C), z(B * T, C)
+            self.chan_ps = S(B * T, ce)
+            self.sw = S(rows_w, C)
+            self.qkv = S(rows_w, 3 * C)
+            self.ao = S(rows_w, C)
+            self.raw = z(B * nW, heads, T, wl)
+            self.o32 = z(rows_w, C)
+            self.xa32 = z(B * L, C)
+            self.q32 = z(B * T, ce)
+            self.xat = S(B * C, L, zero=True)
+            self.kv32 = z(B * C, 2 * ce)
+            self.kchunks = chan_kv_chunks(B * C, ce, L)
+            self.kv_part = z(self.kchunks, B * C, 2 * ce) if self.kchunks > 1 else None
+            self.co32, self.cos = z(B * T, ce), S(B * T, ce)
+            self.t1 = S(B * T, ce)
+            hid = blk.mlp.fc1.out_features
+            self.ws_mlp = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * L, Cdim=C, hidden=hid,
+                                                            nsplit=ns), device)
+            self.ws_mlp_p = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * T, Cdim=C, hidden=hid,
+                                                              nsplit=ns), device)
+        if merge:
+            self.m32 = z(B * L // 4, 4 * C)
+            self.ms = S(B * L // 4, 4 * C)
+            self.logits_ds = z(B, heads, T, T + L // 4)
+            self.rc_up = z(B, T, 2 * C, self.nh, self.nw)
+
+
+def _launch_swin_block(s, w, shift, spa=None):
+    """One SwinTransformerBlock with task prompts (TP:310-405) on the stage space s: s.x [B*L, C] / s.p [B*T, C] are
+    updated in place, s.logits and s.rc receive the block's raw_spa_attn / raw_chan_attn. The last block of the model
+    (w.last) leaves s.p as it is (the plan reads no prompts after it); spa: zeroed [B*T, C] that then receives the
+    window-averaged prompt outputs, which the reference returns as that block's task_prompts (TP:344, :399-405)."""
+    B, T, C, ce = s.B, s.T, s.C, s.ce
+    ops.layernorm(s.x, w.n1w, w.n1b, w.eps, out_f32=s.xn32)                                    # :322
+    ops.layernorm(s.p, w.n1w, w.n1b, w.eps, out_f32=s.pn32)                                    # :317
+    ops.split_f32(s.p, s.ns, out=s.ps)
+    ops.gemm(s.ps, w.tt, bias=w.tt_b, out_split=s.chan_ps)                                     # :319 token_trans
+    ops.swin_window_gather(s.xn32, s.pn32, s.sw, B=B, H=s.H, W=s.W, Cdim=C, T=T, ws=s.ws, shift=shift)   # :326-340
+    ops.gemm(s.sw, w.qkv, bias=w.qkv_b, out_split=s.qkv)                                       # :183
+    ops.swin_window_attention(s.qkv, s.ao, s.raw, w.biasT, w.maskT, BW=B * s.nW, nW=s.nW, T=T, L=s.wl,
+                              heads=s.heads, scale=(C // s.heads) ** -0.5)                      # :185-206
+    ops.gemm(s.ao, w.proj, bias=w.proj_b, out_f32=s.o32)                                       # :207
+    spa_out = w.last and spa is not None
+    ops.swin_window_scatter(s.o32, s.raw, s.xa32, s.x, spa if spa_out else s.p, s.logits, B=B, H=s.H, W=s.W, Cdim=C,
+                            T=T, ws=s.ws, shift=shift, heads=s.heads, last=w.last and not spa_out)  # :210, :343-360, :399
+    # The prompt path -- channel attention between the prompts and the channels of the attention output (:372-396),
+    # then the prompt update and the prompts' own MLP (:403-404) -- is a chain of small launches on B*T rows that
+    # only needs xa: it runs on a side stream next to the MLP of the B*H*W patch rows (:400) and joins at the end.
+    def prompt_path():
+        ops.gemm(s.chan_ps, w.cq, bias=w.cq_b, out_f32=s.q32)
+        ops.transpose_split(s.xa32, s.xat, B=B, L=s.L, Cdim=C)
+        if s.kchunks > 1:   # C rows x (H*W) columns: a handful of M tiles with thousands of K blocks -> split K
+            ops.gemm_splitk(s.xat, w.ckv, s.kv_part, s.kv32, K=s.L, bias=w.ckv_b, chunks=s.kchunks)
+        else:
+            ops.gemm(s.xat, w.ckv, K=s.L, bias=w.ckv_b, out_f32=s.kv32)
+        ops.swin_chan_attention(s.q32, s.kv32, s.co32, s.cos, s.rc, B=B, T=T, Cdim=C, ce=ce, nh=s.nh, nw=s.nw)
+        if not w.last:
+            ops.gemm(s.cos, w.cp, bias=w.cp_b, out_split=s.t1)                                 # chan_proj
+            ops.gemm(s.t1, w.tt1, bias=w.tt1_b, residual=s.p, out_f32=s.p)                     # token_trans1; :403
+            ops.ln_mlp_residual(s.p, w.n2w, w.n2b, w.eps, w.fc1, w.fc1_b, w.fc2, w.fc2_b, s.ws_mlp_p)   # :404
+
+    s.streams.par([prompt_path,
+                   lambda: ops.ln_mlp_residual(s.x, w.n2w, w.n2b, w.eps, w.fc1, w.fc1_b, w.fc2, w.fc2_b, s.ws_mlp)])
+
+
+def _launch_merge(s, w, x_out, p_out):
+    """PatchMerging (TP:430-472) on the stage space s: s.x, s.p, s.logits, s.rc -> x_out [B*L/4, 2C], p_out [B*T, 2C]
+    (fp32), s.logits_ds [B, heads, T, T + L/4] and s.rc_up [B, T, 2C, nh, nw]."""
+    B, T = s.B, s.T
+    ops.swin_merge_gather(s.x, s.m32, B=B, H=s.H, W=s.W, Cdim=s.C)                             # :441-447
+    ops.layernorm(s.m32, w.nw, w.nb, w.eps, out_split=s.ms)
+    ops.gemm(s.ms, w.red, out_f32=x_out)                                                       # :449-450
+    ops.conv3x3_s2_maps(s.logits, w.ds_w, w.ds_b, s.logits_ds, B=B, Cin=s.heads * T, H=s.H, W=s.W,
+                        in_stride=T + s.L, in_offset=T, out_stride=T + s.L // 4, out_offset=T)  # :458-460
+    ops.swin_chan_up(s.rc, w.pca, s.rc_up, BT=B * T, Cdim=s.C, nwin=s.nh * s.nw)               # :463-466
+    ops.split_f32(s.p, s.ns, out=s.ps)
+    ops.gemm(s.ps, w.tpu, out_f32=p_out)                                                       # :469
+
+
+# --------------------------------------------------------------------------------------------
+# the sub-module forwards: the plan's block and merge launches on a workspace sized for the call
+# --------------------------------------------------------------------------------------------
+def _check_tokens(mod, x, prompts, C):
+    """(B, T) of x [B, H*W, C] and task_prompts [B, T, C] for a module over the map `mod.input_resolution`."""
+    H, W = mod.input_resolution if hasattr(mod, "input_resolution") else mod.blocks[0].input_resolution
+    if x.dim() != 3 or tuple(x.shape[1:]) != (H * W, C) or prompts.dim() != 3 or prompts.shape[0] != x.shape[0] \
+            or prompts.shape[2] != C or prompts.shape[1] < 1:
+        raise ValueError(f"{type(mod).__name__}: expected x [B,{H * W},{C}] and task_prompts [B,T,{C}], got "
+                         f"{tuple(x.shape)} and {tuple(prompts.shape)}")
+    return x.shape[0], prompts.shape[1]
+
+
+def _module_space(mod, blk, B, T, dev, ns):
+    """The stage space of a sub-module forward, cached on the module per (device, nsplit, B, T): with the block buffers
+    when blk is given, with the PatchMerging scratch when the module is or has a PatchMerging."""
+    merge = isinstance(mod, PatchMerging) or getattr(mod, "downsample", None) is not None
+    src = blk if blk is not None else mod
+    heads = blk.num_heads if blk is not None else mod.num_heads
+    chan_nheads = src.chan_nheads
+    return _cached(mod, ("space", dev, ns, B, T), lambda: _StageSpace(
+        src.dim, src.input_resolution, heads, B, T, chan_nheads, dev, ns, _Streams(dev, 2), blk=blk, merge=merge),
+        versioned=False)
+
+
+def _load(s, x, prompts):
+    s.x.copy_(x.reshape(s.B * s.L, s.C))
+    s.p.copy_(prompts.reshape(s.B * s.T, s.C))
+
+
+def _attn_out(s, logits, rc, H, W):
+    """[raw_spa_attn [B, heads, T, H, W], raw_chan_attn] (fresh) from the gating-layout logits and the channel logits."""
+    maps = torch.empty(s.B, s.heads, s.T, H, W, device=logits.device, dtype=torch.float32)
+    ops.swin_logit_maps(logits, maps, T=s.T, to_maps=True)
+    return [maps, rc.clone()]
+
+
+def _launch_merge_out(s, w):
+    """PatchMerging on s into fresh tensors: (x [B, L/4, 2C], task_prompts [B, T, 2C], attn_weight)."""
+    B, T, C = s.B, s.T, s.C
+    x = torch.empty(B, s.L // 4, 2 * C, device=s.x.device, dtype=torch.float32)
+    p = torch.empty(B, T, 2 * C, device=s.x.device, dtype=torch.float32)
+    _launch_merge(s, w, x.view(B * s.L // 4, 2 * C), p.view(B * T, 2 * C))
+    return x, p, _attn_out(s, s.logits_ds, s.rc_up, s.H // 2, s.W // 2)
+
+
 class _SwinPlan(Plan):
     """Geometry, workspace and launch sequence of one TaskPrompterSwin wrapper forward. mode: "full" = wrapper forward
     (logits at the output size), "postproc" = predict() (get_output fused into the final resize, same launch count),
@@ -327,47 +556,9 @@ class _SwinPlan(Plan):
             self.cols = S(B * gh * gw, patch * patch * bb.in_chans)
             self.x0 = z(B * gh * gw, E)
             # ---- per stage
-            self.st = []
-            for i, layer in enumerate(bb.layers):
-                C = E * 2 ** i
-                H, W = gh // 2 ** i, gw // 2 ** i
-                blk0 = layer.blocks[0]
-                ws, heads_i = blk0.window_size, blk0.num_heads
-                Hp, Wp = blk0.padded
-                nW = (Hp // ws) * (Wp // ws)
-                L, wl = H * W, ws * ws
-                rows_w = B * nW * (T + wl)
-                s = SimpleNamespace(C=C, H=H, W=W, L=L, ws=ws, heads=heads_i, Hp=Hp, Wp=Wp, nW=nW, wl=wl, rows_w=rows_w)
-                s.x = z(B * L, C)
-                s.p = z(B * T, C)
-                s.xn32, s.pn32 = z(B * L, C), z(B * T, C)
-                s.ps, s.chan_ps = S(B * T, C), S(B * T, ce)
-                s.sw = S(rows_w, C)
-                s.qkv = S(rows_w, 3 * C)
-                s.ao = S(rows_w, C)
-                s.raw = z(B * nW, heads_i, T, wl)
-                s.o32 = z(rows_w, C)
-                s.xa32 = z(B * L, C)
-                s.logits = z(B, heads_i, T, T + L)                 # prompt-row logits in the gating kernel's layout
-                s.q32 = z(B * T, ce)
-                s.xat = S(B * C, L, zero=True)
-                s.kv32 = z(B * C, 2 * ce)
-                s.kchunks = chan_kv_chunks(B * C, ce, L)
-                s.kv_part = z(s.kchunks, B * C, 2 * ce) if s.kchunks > 1 else None
-                s.co32, s.cos = z(B * T, ce), S(B * T, ce)
-                s.t1 = S(B * T, ce)
-                s.rc = z(B, T, C, self.nh, self.nw)
-                hid = layer.blocks[0].mlp.fc1.out_features
-                s.ws_mlp = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * L, Cdim=C, hidden=hid,
-                                                             nsplit=ns), device)
-                s.ws_mlp_p = ops.workspace(ops.workspace_bytes(ops.OP_LN_MLP_RESIDUAL, rows=B * T, Cdim=C, hidden=hid,
-                                                               nsplit=ns), device)
-                if layer.downsample is not None:
-                    s.m32 = z(B * L // 4, 4 * C)
-                    s.ms = S(B * L // 4, 4 * C)
-                    s.logits_ds = z(B, heads_i, T, T + L // 4)
-                    s.rc_up = z(B, T, 2 * C, self.nh, self.nw)
-                self.st.append(s)
+            self.st = [_StageSpace(b0.dim, b0.input_resolution, b0.num_heads, B, T, p.chan_nheads, device, ns, self.streams,
+                                   blk=b0, merge=layer.downsample is not None)
+                       for layer, b0 in ((layer, layer.blocks[0]) for layer in bb.layers)]
             last = self.st[-1]
             self.xfin = z(B * last.L, last.C)
             # ---- decoder levels: level il lives on the map AFTER stage il's merging (the last level: the final norm)
@@ -418,53 +609,6 @@ class _SwinPlan(Plan):
         return {t: list(self.det_out) if t == DET else self.out[t] for t in self.tasks}
 
     # ------------------------------------------------------------------------------------------
-    def _block(self, s, w, blk):
-        """One SwinTransformerBlock with task prompts (TP:310-405) on stage buffers s.x [B*L, C] / s.p [B*T, C]."""
-        B, T, C, ce = self.B, self.T, s.C, self.ce
-        shift = blk.shift_size
-        ops.layernorm(s.x, w.n1w, w.n1b, w.eps, out_f32=s.xn32)                                    # :322
-        ops.layernorm(s.p, w.n1w, w.n1b, w.eps, out_f32=s.pn32)                                    # :317
-        ops.split_f32(s.p, self.ns, out=s.ps)
-        ops.gemm(s.ps, w.tt, bias=w.tt_b, out_split=s.chan_ps)                                     # :319 token_trans
-        ops.swin_window_gather(s.xn32, s.pn32, s.sw, B=B, H=s.H, W=s.W, Cdim=C, T=T, ws=s.ws, shift=shift)   # :326-340
-        ops.gemm(s.sw, w.qkv, bias=w.qkv_b, out_split=s.qkv)                                       # :183
-        ops.swin_window_attention(s.qkv, s.ao, s.raw, w.biasT, w.maskT, BW=B * s.nW, nW=s.nW, T=T, L=s.wl,
-                                  heads=s.heads, scale=(C // s.heads) ** -0.5)                      # :185-206
-        ops.gemm(s.ao, w.proj, bias=w.proj_b, out_f32=s.o32)                                       # :207
-        ops.swin_window_scatter(s.o32, s.raw, s.xa32, s.x, s.p, s.logits, B=B, H=s.H, W=s.W, Cdim=C, T=T, ws=s.ws,
-                                shift=shift, heads=s.heads, last=w.last)                            # :210, :343-360, :399
-        # The prompt path -- channel attention between the prompts and the channels of the attention output (:372-396),
-        # then the prompt update and the prompts' own MLP (:403-404) -- is a chain of small launches on B*T rows that
-        # only needs xa: it runs on a side stream next to the MLP of the B*H*W patch rows (:400) and joins at the end.
-        def prompt_path():
-            ops.gemm(s.chan_ps, w.cq, bias=w.cq_b, out_f32=s.q32)
-            ops.transpose_split(s.xa32, s.xat, B=B, L=s.L, Cdim=C)
-            if s.kchunks > 1:   # C rows x (H*W) columns: a handful of M tiles with thousands of K blocks -> split K
-                ops.gemm_splitk(s.xat, w.ckv, s.kv_part, s.kv32, K=s.L, bias=w.ckv_b, chunks=s.kchunks)
-            else:
-                ops.gemm(s.xat, w.ckv, K=s.L, bias=w.ckv_b, out_f32=s.kv32)
-            ops.swin_chan_attention(s.q32, s.kv32, s.co32, s.cos, s.rc, B=B, T=T, Cdim=C, ce=ce, nh=self.nh, nw=self.nw)
-            if not w.last:
-                ops.gemm(s.cos, w.cp, bias=w.cp_b, out_split=s.t1)                                 # chan_proj
-                ops.gemm(s.t1, w.tt1, bias=w.tt1_b, residual=s.p, out_f32=s.p)                     # token_trans1; :403
-                ops.ln_mlp_residual(s.p, w.n2w, w.n2b, w.eps, w.fc1, w.fc1_b, w.fc2, w.fc2_b, s.ws_mlp_p)   # :404
-
-        self.streams.par([prompt_path,
-                          lambda: ops.ln_mlp_residual(s.x, w.n2w, w.n2b, w.eps, w.fc1, w.fc1_b, w.fc2, w.fc2_b, s.ws_mlp)])
-
-    def _merge(self, i):
-        """PatchMerging (TP:430-472): stage i -> the inputs of stage i + 1 and of decoder level i."""
-        B, T = self.B, self.T
-        s, n, w = self.st[i], self.st[i + 1], self.Wm[i]
-        ops.swin_merge_gather(s.x, s.m32, B=B, H=s.H, W=s.W, Cdim=s.C)                             # :441-447
-        ops.layernorm(s.m32, w.nw, w.nb, w.eps, out_split=s.ms)
-        ops.gemm(s.ms, w.red, out_f32=n.x)                                                         # :449-450
-        ops.conv3x3_s2_maps(s.logits, w.ds_w, w.ds_b, s.logits_ds, B=B, Cin=s.heads * T, H=s.H, W=s.W,
-                            in_stride=T + s.L, in_offset=T, out_stride=T + s.L // 4, out_offset=T)  # :458-460
-        ops.swin_chan_up(s.rc, w.pca, s.rc_up, BT=B * T, Cdim=s.C, nwin=self.nh * self.nw)         # :463-466
-        ops.split_f32(s.p, self.ns, out=s.ps)
-        ops.gemm(s.ps, w.tpu, out_f32=n.p)                                                         # :469
-
     def _level(self, il, x_src, logits, rc):
         """cal_task_feature (TP:721-774) at level il on X = x_src [B*P, C]."""
         B, T, d = self.B, self.T, self.lv[il]
@@ -541,10 +685,10 @@ class _SwinPlan(Plan):
         n_stage = len(self.st)
         for i, s in enumerate(self.st):
             for j, blk in enumerate(bb.layers[i].blocks):
-                self._block(s, self.Wb[i][j], blk)
+                _launch_swin_block(s, self.Wb[i][j], blk.shift_size)
             if i < n_stage - 1:
-                self._merge(i)
                 n = self.st[i + 1]
+                _launch_merge(s, self.Wm[i], n.x, n.p)                                             # stage i -> i + 1
                 self._level(i, n.x, s.logits_ds, s.rc_up)                                          # :702-707
         last = self.st[-1]
         ops.layernorm(last.x, W.nw, W.nb, W.neps, out_f32=self.xfin)                               # :709
